@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py - BN254 G1 MSM throughput (BASELINE.json metric, configs[1]) on N B200s, plus the other BASELINE
+"""bench.py - BN254 G1 MSM throughput (BASELINE.json metric, configs[1]) on N H100s, plus the other BASELINE
 configs as secondary legs of the same JSON line.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]          # this repo's CUDA path
+  python bench.py --dump-outputs DIR [...]                      # also write the last timed step's result as DIR/*.npy
   python bench.py --impl reference [...]                        # CPU arm (oracle port, all host cores)
   torchrun --nproc-per-node N bench.py --gpus N ...             # one rank per GPU
 
@@ -46,8 +47,7 @@ CONFIG = {"workload": "BN254 G1 MSM, 2^20 uniform random scalars x 2^20 distinct
           "curve": "bn254", "group": "G1", "points_per_gpu": 1 << LOG_N}
 LEG_LIMIT_S = {"strong": 240, "groth16": 300, "plonk": 420, "bw6": 300}
 WHOLE_RUN_LIMIT_S = 1500
-LOAD_STEPS = 160   # fixed-count load phase (>= 0.5 s at ~3.5 ms / MSM) so that nvidia-smi's 100 ms sampler sees clocks under load
-NCU_TRAFFIC_FILE = os.path.join(ROOT, "profiles", "ncu_accumulate_traffic.json")
+LOAD_STEPS = 160   # fixed-count load phase (>= 0.5 s at a few ms / MSM) so that nvidia-smi's 100 ms sampler sees clocks under load
 
 
 # --------------------------------------------------------------------------------------
@@ -90,7 +90,7 @@ def jac_to_affine(C, jac, group=1):
 
 # --------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -137,37 +137,30 @@ class ClockSampler:
                 "samples": len(sm), "samples_under_load": len(busy)}
 
 
-IMAD_WIDE_LANES_PER_CLK_SM = 32   # measured issue rate of IMAD.WIDE (half-rate pipe), profiles/r01_microbench_pipes.txt
-N_SMS = 148
+IMAD_WIDE_LANES_PER_CLK_SM = 32   # IMAD.WIDE issues at half the IMAD rate, 64 lanes/clk/SM on H100 (tools/microbench.cu)
+HBM_PEAK_GBS = 3350.0             # H100 SXM data sheet (HBM3)
 
 
-def multiplier_roofline(entries, imad_per_entry, kernel_ms, clocks):
-    mhz = (clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1965.0
-    peak = N_SMS * IMAD_WIDE_LANES_PER_CLK_SM * mhz * 1e6 / 1e12
+def multiplier_roofline(entries, imad_per_entry, kernel_ms, clocks, sms):
+    mhz = (clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1980.0   # H100 SXM boost clock
+    peak = sms * IMAD_WIDE_LANES_PER_CLK_SM * mhz * 1e6 / 1e12
     achieved = entries * imad_per_entry / (kernel_ms / 1e3) / 1e12
     return {"bound": "int32 multiplier issue", "achieved": achieved, "peak": peak, "unit": "T IMAD.WIDE/s",
             "frac": achieved / peak, "sm_mhz": mhz, "imad_wide_per_bucket_entry": imad_per_entry,
             "model": "bucket entries x IMAD.WIDE per XYZZ mixed addition (static SASS count) / accumulate time; "
-                     "peak = 148 SMs x 32 lanes/clk x SM clock under load"}
+                     f"peak = {sms} SMs x {IMAD_WIDE_LANES_PER_CLK_SM} lanes/clk x SM clock under load"}
 
 
-def measured_peak_gbs():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+def dump_outputs(out_dir, arrays):
+    """write each array as out_dir/<name>.npy in float64 (exact: every value is a 32-bit word)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
 
 
-def ncu_traffic():
-    """dram bytes of one k_msm_accumulate launch from the committed ncu --set full capture (profiles/), or None"""
-    try:
-        d = json.load(open(NCU_TRAFFIC_FILE))
-        return float(d["dram_bytes_per_launch"]), d.get("source", NCU_TRAFFIC_FILE)
-    except Exception:
-        return None, None
+def u32_words(values, nwords):
+    """non-negative ints -> (len(values), nwords) little-endian 32-bit words"""
+    return np.array([[(v >> (32 * k)) & 0xFFFFFFFF for k in range(nwords)] for v in values], dtype=np.uint64)
 
 
 # --------------------------------------------------------------------------------------
@@ -372,8 +365,14 @@ def msm_leg(ctx):
     for _ in range(LOAD_STEPS // K + 1):     # fixed count on every rank
         run_steps(K)
     ms, _ = timed_region(ctx, lambda: run_steps(K))
-    got = jac_to_affine(C, d_tot[K - 1].cpu().numpy().view(np.uint64))
+    last = d_tot[K - 1].cpu().numpy().view(np.uint64)
+    got = jac_to_affine(C, last)
     assert got == expected_total, "sum over ranks does not match the known-discrete-log oracle"
+    if args.dump_outputs and rank == 0:
+        # the Jacobian point the caller receives (X, Y, Z in Montgomery form, as 32-bit words) and the same point in
+        # canonical affine coordinates, which two builds agree on even where their Jacobian representatives differ
+        dump_outputs(args.dump_outputs, {"msm_result_jacobian": last.view(np.uint32).reshape(3, 8),
+                                         "msm_result_affine": u32_words(got, 8)})
 
     # ---- end to end through the C ABI with HOST buffers (e2e) -------------------------------------------
     # K x b200_msm_submit_dev (pinned host scalars: H2D on the copy stream, overlapped with the previous MSM), one
@@ -411,12 +410,11 @@ def msm_leg(ctx):
 
     total = n * world
     value = total * K / (ms / 1e3)
-    peak, peak_src = measured_peak_gbs()
     Wn = info["n_windows"]
     alg_bytes = n * Wn * (64 + 4)           # SURVEY.md §8d: W x (sizeof(affine) + 4 B index) per scalar-mul
     acc_ms = stage_ms["accumulate"]
     achieved = alg_bytes / (acc_ms / 1e3) / 1e9
-    traffic, traffic_src = ncu_traffic()
+    sms = torch.cuda.get_device_properties(local).multi_processor_count
     out = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": DTYPE,
@@ -426,7 +424,7 @@ def msm_leg(ctx):
                     "parallelism": (f"point-range shard x{world}: one ncclAllGather of K x {world} partial points + fold kernel "
                                     "on the device (b200_points_allreduce)") if world > 1 else "single GPU",
                     "l2": "no flush: per-step working set (table %.2f GiB gathered at random + scalars 32 MiB + 256 MiB sort "
-                          "buffers) exceeds the 126 MB L2" % (info["device_bytes"] / 2**30)},
+                          "buffers) exceeds the 50 MB L2" % (info["device_bytes"] / 2**30)},
         "e2e": {"value": total * K / e2e_s, "unit": UNIT, "h2d_bytes_per_step": n * 32 * world, "d2h_bytes_per_step": 96 * world,
                 "ms_per_step": 1e3 * e2e_s / K,
                 "note": "K x b200_msm_submit_dev from pinned host scalars (upload overlapped with the previous MSM), combine, "
@@ -436,10 +434,10 @@ def msm_leg(ctx):
         # own kernels per MSM: decompose, bucket_offsets, task_counts, accumulate, combine, combine_heavy,
         # reduce_chunks, set_sum, finish (the radix sort and the scans are CUB launches on top of these)
         "gpu_launches": 9 * K + (1 if world > 1 else 0),
-        "roofline": {"bound": "hbm", "kernel": "k_msm_accumulate", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
-                     "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": acc_ms, "traffic_source": traffic_src,
-                     "multiplier": multiplier_roofline(n * Wn, args.imad_per_add, acc_ms, clocks),
+        "roofline": {"bound": "hbm", "kernel": "k_msm_accumulate", "achieved": achieved, "peak": HBM_PEAK_GBS, "unit": "GB/s",
+                     "frac": achieved / HBM_PEAK_GBS, "peak_source": "H100 SXM data sheet",
+                     "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": acc_ms,
+                     "multiplier": multiplier_roofline(n * Wn, args.imad_per_add, acc_ms, clocks, sms),
                      "note": "integer-multiplier bound, not HBM bound: >1000 IMAD.WIDE per gathered 68 B (DESIGN.md §3)"},
         "stage_ms": stage_ms,
         "clocks": clocks,
@@ -733,7 +731,9 @@ def main():
     ap.add_argument("--bw6", action="store_true", default=None, help="BW6-761 G1 MSM 2^24 sharded (configs[4]); default: at N=8")
     ap.add_argument("--bw6-log", type=int, default=24)
     ap.add_argument("--imad-per-add", type=int, default=1360,
-                    help="IMAD.WIDE per XYZZ mixed addition of the shipped kernel (static SASS count, profiles/)")
+                    help="IMAD.WIDE per XYZZ mixed addition of the shipped kernel (static SASS count, tools/sass_stats.py)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the headline MSM result of the last step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     dog = arm_watchdog(WHOLE_RUN_LIMIT_S, code=1)
     if args.impl == "reference":

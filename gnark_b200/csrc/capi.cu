@@ -72,10 +72,9 @@ int32_t device_ctx(int dev, DeviceCtx** out) {
     uint64_t thr = UINT64_MAX;  // keep freed workspace cached in the pool
     CK(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
     // L2 fill granularity on a miss: 64 bytes.  The bucket accumulate gathers 64-byte (BN254 G1) / 96..192-byte points at
-    // random from a table far larger than L2; with the driver's default (128) ncu shows 2.33 GB of DRAM traffic for
-    // 1.14 GB of gathered points, with 64 it is 1.24 GB (profiles/r02_session4.md).  The kernels are multiplier-bound,
-    // so the time does not move - this removes wasted HBM traffic, nothing else.  GB200_L2_FETCH=32|64|128 overrides, 0 leaves
-    // the device limit alone.
+    // random from a table far larger than L2; with the driver's default (128) every 64-byte gather drags a second sector
+    // in with it.  The kernels are multiplier-bound, so the time does not move - this removes wasted HBM traffic, nothing
+    // else.  GB200_L2_FETCH=32|64|128 overrides, 0 leaves the device limit alone.
     if (const int g = env_int("GB200_L2_FETCH", 64)) CK(cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g));
     c.dev = dev;
     c.ready = true;
@@ -101,16 +100,15 @@ void msm_tuning(size_t n, int nwin, int c, int precomp, int acc_blocks_per_sm, u
   const size_t buckets = (precomp ? (size_t)1 : (size_t)nwin) << (c - 1);
   // Task length.  One thread adds a task's entries; a bucket of k entries is cut into ceil(k / task_len) tasks.  Short
   // tasks fill the machine evenly (the accumulate grid is many waves deep, the short last task of every bucket idles its
-  // lane for less) at the price of more partial sums for the combine kernel.  Measured on B200 (round 2, BN254 G1 2^20,
-  // pipelined ms per MSM): 16: 3.50, 24: 3.42, 32: 3.43, 40: 3.45, 48: 3.49, 64: 3.54; BN254 G2 / BLS12-381 G1: 32 beats
-  // 64 by 4-5 %.  Within [24, 40] ([48, 64] for grids of a dozen waves and more) the length is picked so that the grid is as close as possible to a whole number of
-  // waves of resident blocks (148 SMs x blocks per SM from the occupancy API): the last, partly filled wave is the
-  // other loss (BW6-761 2^18 with 64-entry tasks: 3.04 waves of 296 blocks, a quarter of the kernel's time on 4 % of it).
-  int sms = 148;
+  // lane for less) at the price of more partial sums for the combine kernel.  Within [24, 40] ([48, 64] for grids of a
+  // dozen waves and more) the length is picked so that the grid is as close as possible to a whole number of waves of
+  // resident blocks (the device's SMs - 132 on H100 SXM - x blocks per SM from the occupancy API): the last, partly
+  // filled wave is the other loss (a grid of 3.04 waves spends a quarter of the kernel's time on 4 % of its work).
+  int sms = 132;
   { int dev = 0; if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   const double resident = (double)sms * (acc_blocks_per_sm > 0 ? acc_blocks_per_sm : 1);
   // a grid a dozen waves deep loses little to its last wave: there the longer task wins again, because every partial
-  // costs the combine kernel one full addition (2^24 points, 64-entry tasks: combine 3.2 of 50 ms; at 40 entries 5 ms)
+  // costs the combine kernel one full addition
   const double waves64 = ((double)m / 64.0 + 0.5 * (double)buckets) / 128.0 / resident;
   size_t lo = waves64 >= 12.0 ? 48 : 24, hi = waves64 >= 12.0 ? 64 : 40;
   const size_t per_bucket = m / (buckets ? buckets : 1);
@@ -201,7 +199,7 @@ using namespace gb200;
 
 extern "C" {
 
-const char* b200_version(void) { return "gnark_b200 0.1.0 (sm_100a)"; }
+const char* b200_version(void) { return "gnark_b200 0.1.0 (sm_90a)"; }
 const char* b200_last_error(void) { return g_last_error.c_str(); }
 
 int32_t b200_device_count(int32_t* out) {

@@ -1,4 +1,4 @@
-// Prime-field arithmetic in Montgomery form, 32-bit limbs, for sm_100a.
+// Prime-field arithmetic in Montgomery form, 32-bit limbs, for sm_90a.
 //
 // Memory layout is gnark-crypto's fp.Element / fr.Element bit for bit
 // ([Limbs]uint64 little-endian, value x*R mod q, R = 2^(64*Limbs); SURVEY.md
@@ -86,8 +86,8 @@ HD void mont_mul_raw(uint32_t* r, const uint32_t* a, const uint32_t* b) {
 
 // ---------------------------------------------------------------------------
 // Wide (unreduced) products and a separate Montgomery reduction: the building blocks of the lazily reduced Fp2 product
-// (Fp2::mul_lazy: 3 wide products + 2 reductions instead of 3 + 3; measured on B200, round 2: BN254 G2 accumulate
-// 11.4 -> 10.2 ms).  Bit-exact against the fused product (tests/test_emulation.py::test_wide_arithmetic).
+// (Fp2::mul_lazy: 3 wide products + 2 reductions instead of 3 + 3).  Bit-exact against the fused product
+// (tests/test_emulation.py::test_wide_arithmetic).
 // ---------------------------------------------------------------------------
 
 // t[0..2N) = a * b for ANY N-limb a, b (no reduction).  Same even/odd carry chains as mont_mul_raw without the m*p rows.
@@ -232,8 +232,7 @@ struct alignas(16) Fp {
   HD friend Fp operator-(const Fp& a, const Fp& b) { Fp r; mod_sub_raw<P>(r.l, a.l, b.l); return r; }
   // Fields of up to 8 limbs get the product inlined at every use; larger ones keep ONE copy of the unrolled product per
   // kernel (I-cache, compile time), called with operands and result in REGISTERS: a reference parameter makes the
-  // caller spill both operands to its stack frame and the callee load them back (round-2 A/B on B200: BLS12-381 G1
-  // accumulate 8.39 -> 6.75 ms, BW6-761 18.4 -> 12.6 ms, BN254 G2 11.4 -> 10.0 ms with operands by value).
+  // caller spill both operands to its stack frame and the callee load them back.
   static constexpr int INLINE_LIMBS = 8;
 #if defined(__CUDA_ARCH__)
   static __device__ __noinline__ Fp mul_ni(Fp a, Fp b) { Fp r; mont_mul_raw<P>(r.l, a.l, b.l); return r; }

@@ -1,4 +1,4 @@
-// Groth16 prover host layer: the B200 twin of
+// Groth16 prover host layer: the GPU twin of
 // backend/accelerated/icicle/groth16/bn254/icicle.go (setupDevicePointers :88-264,
 // Prove :784-1360, computeH :1391-1488) and of the CPU prover
 // backend/groth16/bn254/prove.go:52-315, from "solved witness" to "proof points".

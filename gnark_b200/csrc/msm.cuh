@@ -1,4 +1,4 @@
-// Pippenger bucket MSM - per-thread logic (host/device) shared by the sm_100a
+// Pippenger bucket MSM - per-thread logic (host/device) shared by the sm_90a
 // kernels in msm_impl.cuh and by the CPU emulation used in the "not gpu" tests.
 //
 // Replaces gnark-crypto's G1Jac/G2Jac.MultiExp at the reference's call sites
@@ -18,7 +18,7 @@
 //                 tree sum; Horner over bucket sets when there is more than one.
 //
 // Table modes.  PRECOMP: the device table holds 2^(c*w)*P_i for every window w
-// (layout [w][i], built once at table upload - HBM3e capacity traded for the
+// (layout [w][i], built once at table upload - HBM capacity traded for the
 // removal of the serial 2^c-doubling Horner tail and of W-1 bucket reductions):
 // all windows share ONE bucket set.  PLAIN: table = the n points; W bucket sets.
 #pragma once

@@ -1,4 +1,4 @@
-// sm_100a kernels + stream-ordered host driver for the bucket MSM (see msm.cuh for
+// sm_90a kernels + stream-ordered host driver for the bucket MSM (see msm.cuh for
 // the algorithm and the reference call sites it replaces).
 #pragma once
 #include <cub/cub.cuh>
@@ -48,9 +48,9 @@ static __global__ void k_msm_task_counts(const uint32_t* __restrict__ off, uint3
 
 // one thread per task: partial[t] = sum of <= task_len consecutive entries of one bucket
 // Resident blocks per SM asked of ptxas (register cap 65536 / (128 k)); 1 = the compiler's own allocation.
-// 64-byte coordinates (Fp2 over 8 limbs, BN254 G2): left alone ptxas takes 224 registers = 2 blocks / SM and the IMAD pipe
-// sits at 77 %; capped at 168 registers (3 blocks / SM, 212 bytes of spills) the kernel is 7 % faster (8.46 -> 7.89 ms
-// at 2^20, profiles/r02_session4.md).  96-byte coordinates (Fp2 over 12 limbs, BW6-761 Fp) already spill at 255
+// 64-byte coordinates (Fp2 over 8 limbs, BN254 G2): left alone ptxas takes over 200 registers = 2 blocks / SM; capped at
+// 168 registers (3 blocks / SM) a few spills buy a third resident block, which keeps the IMAD pipe busier while
+// one block waits on its gathers.  96-byte coordinates (Fp2 over 12 limbs, BW6-761 Fp) already spill at 255
 // registers = 2 blocks / SM and are left alone.
 #ifndef GB200_ACC_MIN_BLOCKS_64
 #define GB200_ACC_MIN_BLOCKS_64 3
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(128) k_msm_reduce_chunks(MsmPlan pl, uint32_t 
   chunk_sums[g] = msm_reduce_chunk<F>(buckets + (size_t)s * pl.set_size, lo, hi);
 }
 
-// The tail is a chain of dependent point additions (5-7 us each on an otherwise idle SM), so its cost is its DEPTH: the
+// The tail is a chain of dependent point additions (microseconds each on an otherwise idle SM), so its cost is its DEPTH: the
 // chunk sums of a set are added as a pure tree - block (slice, set) reduces one slice of them in shared memory, one entry
 // per thread where the slice allows, k_msm_finish adds the slice sums - 12 levels for 4096 chunk sums.
 template <class F>
@@ -361,7 +361,7 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
                         const MsmPipe* pipe = nullptr) {
   // pipe (optional, internal.h): the accumulate kernel and the latency-bound reduction kernels that follow it are
   // enqueued on their own streams (forked with events), so that in a pipeline of MSMs the next MSM's DRAM-bound
-  // front overlaps this one's multiplier-bound accumulate, and the tail overlaps both instead of idling 140+ SMs.
+  // front overlaps this one's multiplier-bound accumulate, and the tail overlaps both instead of idling most of the SMs.
   // ev (optional, MSM_NUM_EVENTS entries): stage boundaries for the step profile
   // (the reference's ICICLE_STEP_PROFILE timers, icicle.go:72-75,1088-1094)
 #define GB_EV(k) do { if (ev) GB_CUDA_TRY(cudaEventRecord(ev[k], stream)); } while (0)
@@ -418,7 +418,10 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
     const int ht = 128;  // 4 warps = 4 buckets in flight per block
     const size_t hsmem = (size_t)ht * sizeof(XYZZ<F>);
     GB_CUDA_TRY(cudaFuncSetAttribute(k_msm_combine_heavy<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsmem));
-    k_msm_combine_heavy<F><<<148 * 2, ht, hsmem, stream>>>(task_off, partial, buckets, heavy, heavy + 1);
+    int dev = 0, sms = 132;    // two blocks per SM (132 on H100 SXM)
+    GB_CUDA_TRY(cudaGetDevice(&dev));
+    GB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    k_msm_combine_heavy<F><<<sms * 2, ht, hsmem, stream>>>(task_off, partial, buckets, heavy, heavy + 1);
   }
   GB_EV(5);
   const uint32_t nchunks = L.chunks_per_set * (uint32_t)pl.nsets;

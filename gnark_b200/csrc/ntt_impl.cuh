@@ -1,4 +1,4 @@
-// sm_100a NTT kernels + device domain + stream-ordered drivers (see ntt.cuh for the
+// sm_90a NTT kernels + device domain + stream-ordered drivers (see ntt.cuh for the
 // conventions and the reference call sites), plus the fused Groth16 quotient
 // pipeline computeH (backend/groth16/bn254/prove.go:346-389, GPU twin
 // backend/accelerated/icicle/groth16/bn254/icicle.go:1391-1488).
@@ -85,8 +85,8 @@ k_ntt_pass(NttPass p, int logn, int dit, const Fr* __restrict__ tw, Fr* __restri
     }
 #pragma unroll
     for (int l = 0; l < N; l++) { sm[l * tile_elems + lo] = a.l[l]; sm[l * tile_elems + hi] = b.l[l]; }
-    // (between two stages on local bits <= 5 a warp only touches its own 64 slots and __syncwarp() would do; measured
-    // 1 % slower than the block barrier, profiles/r02_session5.md)
+    // (between two stages on local bits <= 5 a warp only touches its own 64 slots and __syncwarp() would do; it was
+    // not faster than the block barrier)
     __syncthreads();
   }
 
@@ -143,11 +143,11 @@ struct NttDomainDev {
     n = 1u << logn;
     // Tile = 2^8 elements (128 threads, 8 KiB of shared memory per block): a pass is a chain of barrier-separated phases
     // (load, one stage per barrier, store), so SMALL blocks - many resident per SM - overlap one block's loads and
-    // barriers with another's butterflies.  Measured on B200 (round 2, tools/sweep_ntt.py, ms per transform):
+    // barriers with another's butterflies.  Measured on H100 SXM (400 W power limit; tools/sweep_ntt.py, ms per transform):
     //   tile            2^11    2^10    2^9     2^8     2^7
-    //   BN254 2^20      0.327   0.255   0.229   0.216   0.220     (2^11: one 1024-thread block per SM, IMAD pipe at 45 %)
-    //   BN254 2^24      5.54    4.58    4.03    3.79    3.82
-    //   BLS12-381 2^22  1.49    1.23    1.02    0.977   0.968
+    //   BN254 2^20      0.316   0.292   0.255   0.238   0.248     (2^11: one 1024-thread block per SM)
+    //   BN254 2^24      6.17    5.55    5.39    4.94    5.18
+    //   BLS12-381 2^22  1.55    1.31    1.17    1.15    1.14
     // although the smaller tiles need more passes (2^20: 2 passes at 2^11, 3 at 2^9 / 2^8).  GB200_NTT_TILE_LOG (6..11) overrides.
     int tile_log = NTT_DEFAULT_TILE_LOG;
     if (const char* e = getenv("GB200_NTT_TILE_LOG")) { const int v = atoi(e); if (v >= 6 && v <= NTT_MAX_TILE_LOG) tile_log = v; }

@@ -1,4 +1,4 @@
-// Carry-chain primitives: PTX mad.lo.cc / madc.hi.cc / add.cc / sub.cc on sm_100a,
+// Carry-chain primitives: PTX mad.lo.cc / madc.hi.cc / add.cc / sub.cc on sm_90a,
 // with a bit-exact host emulation (explicit carry flag) so that the SAME field /
 // curve templates can be unit-tested on a CPU-only box (tests/, -m "not gpu").
 // The host path is test scaffolding for the arithmetic templates, not a product

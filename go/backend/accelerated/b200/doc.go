@@ -1,4 +1,4 @@
-// Package b200 implements accelerated prover backends for NVIDIA B200 (sm_100a) on top of libgnark_b200.so.
+// Package b200 implements accelerated prover backends for NVIDIA H100 (sm_90a) on top of libgnark_b200.so.
 //
 // The package layout, the function sets and the option handling follow
 // [github.com/consensys/gnark/backend/accelerated/icicle] one to one, so that switching is an import change:

@@ -1,4 +1,4 @@
-/* libgnark_b200.so - C ABI of the B200 (sm_100a) prover-arithmetic backend for gnark.
+/* libgnark_b200.so - C ABI of the H100 (sm_90a) prover-arithmetic backend for gnark.
  *
  * This is the drop-in boundary for the Groth16 / PLONK prover hot path: every
  * entry point below is what a cgo shim package backend/accelerated/b200/... would

@@ -22,7 +22,7 @@ def test_exports(b200lib):
         assert hasattr(b200lib, s), f"{s} declared in include/gnark_b200.h but not exported"
     from gnark_b200 import lib
     assert set(lib.EXPORTS) == set(syms)
-    assert b"sm_100a" in b200lib.b200_version()
+    assert b"sm_90a" in b200lib.b200_version()
 
 
 def test_no_cpu_fallback(b200lib):

@@ -1,4 +1,4 @@
-"""GPU tests of the entry points added late in round 1 (all of them ran green on a B200 in round 2, unguarded).
+"""GPU tests of the entry points added late in round 1 (all of them run unguarded on an H100).
 
   * test_cuda_reproduces_golden   - the CUDA path on the committed known-answer vectors (tests/golden)
   * test_cuda_reproduces_eth_kzg_srs - the CUDA path on the reference's external fixture (Ethereum KZG ceremony SRS)

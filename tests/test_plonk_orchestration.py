@@ -5,7 +5,7 @@ patches, coset handles, slice arithmetic and the linearised-polynomial / batch-o
 backend/plonk/bn254/prove.go:404-837 - against oracle/plonk_prover.py with the same injected challenges.
 
 The C-ABI entry points themselves are pinned on hardware by tests/test_gpu_plonk.py; the two together are
-what tests/test_gpu_zz_late.py::test_full_prover_vs_oracle checks in one piece on a B200.  Nothing here is a
+what tests/test_gpu_zz_late.py::test_full_prover_vs_oracle checks in one piece on an H100.  Nothing here is a
 product code path: the mock lives in this test file only.
 """
 import contextlib

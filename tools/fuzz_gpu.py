@@ -4,7 +4,7 @@ NTT sizes / modes, computeH, fixed-base batches and gather-index MSMs through th
 the C++ oracle (oracle/c/oracle.cpp) on the same seeded input.  Test infrastructure (it imports oracle/); the fixed
 cases live in tests/test_gpu_*.py, this tool widens them with sizes and patterns nobody picked by hand.
 
-    python tools/fuzz_gpu.py --seconds 300 --seed 1 > gpurun_out/fuzz_gpu.jsonl
+    python tools/fuzz_gpu.py --seconds 300 --seed 1 > fuzz_gpu.jsonl
 
 One JSON line per case class at the end (cases run, failures with their reproducer seeds); exit code 1 on any mismatch.
 """

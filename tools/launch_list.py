@@ -2,7 +2,7 @@
 """Markdown table of ONE MSM's launches from an `ncu --metrics gpu__time_duration.sum --csv` launch list of bench.py:
 the launches between the last two k_msm_decompose, with each kernel's share of their sum.
 
-   python tools/launch_list.py gpurun_out/launches.csv > profiles/rNN_launches_<what>.md"""
+   python tools/launch_list.py launches.csv > launches_<what>.md"""
 import csv
 import re
 import sys

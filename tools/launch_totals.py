@@ -2,7 +2,7 @@
 """Per-kernel totals of an `ncu --metrics gpu__time_duration.sum --csv` launch list, from the launch that matches
 `--from <kernel substring>` (its LAST-BUT-k occurrence, default: first) to the end: count, total ms, share.
 
-   python tools/launch_totals.py gpurun_out/launches_plonk.csv --from k_plonk_ratio --nth -1"""
+   python tools/launch_totals.py launches_plonk.csv --from k_plonk_ratio --nth -1"""
 import argparse
 import csv
 import re

@@ -1,6 +1,6 @@
 // Pipe-throughput microbenchmark for the integer-multiplier question behind the MSM roofline:
-// how many IMAD / IMAD.WIDE / IMAD.HI / DFMA warp-instructions per clock per SM does B200 issue,
-// and do DFMA and IMAD overlap?  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench microbench.cu
+// how many IMAD / IMAD.WIDE / IMAD.HI / DFMA warp-instructions per clock per SM does H100 issue,
+// and do DFMA and IMAD overlap?  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench microbench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -104,8 +104,8 @@ int main() {
     double ops = (double)blocks * threads * ITER * CHAINS;  // lane-ops
     auto rep = [&](const char* name, float ms, double per_iter) {
       double lane_per_s = ops * per_iter / (ms * 1e-3);
-      printf("  %-22s warps/SM=%2d  %8.3f ms  %7.2f Tlane-op/s  = %6.1f lane-op/clk/SM @1.9GHz\n", name, warps_per_sm, ms,
-             lane_per_s / 1e12, lane_per_s / sms / 1.9e9);
+      printf("  %-22s warps/SM=%2d  %8.3f ms  %7.2f Tlane-op/s  = %6.1f lane-op/clk/SM at the nominal clock\n", name,
+             warps_per_sm, ms, lane_per_s / 1e12, lane_per_s / sms / (clk_khz * 1e3));
     };
     rep("IMAD lo", timeit([&] { k_imad_lo<<<blocks, threads>>>(out, 3, 5); }), 1);
     rep("IMAD.HI", timeit([&] { k_imad_hi<<<blocks, threads>>>(out, 3, 5); }), 1);

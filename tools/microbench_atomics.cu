@@ -1,10 +1,10 @@
 // Micro-benchmark for a counting-sort front of the MSM (the question: can 2 x 16.7 M global atomics on 32 K counters
-// beat the two CUB onesweep passes, 0.31 ms?).  m entries with pseudo-random 15-bit keys:
+// beat the two CUB onesweep passes?).  m entries with pseudo-random 15-bit keys:
 //   (a) histogram: red.global.add on hist[key]                       (no return value)
 //   (b) scatter:   pos = atomicAdd(&cursor[key], 1); out[pos] = val  (return value + scattered 4-byte store)
 //   (c) the same two with every key equal (fully skewed input)
 //   (d) block-local shared-memory histogram of 32 K bins (128 KB) flushed with global reds
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/microbench_atomics tools/microbench_atomics.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/microbench_atomics tools/microbench_atomics.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -83,7 +83,9 @@ int main() {
            [&](bool prep) { if (prep) set_cursor(skew); else k_scatter<<<blocks, 256>>>(m, nb - 1, skew, cursor, out); });
   }
   cudaFuncSetAttribute(k_hist_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(nb * 4));
-  for (int g : {148, 296}) {
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  for (int g : {sms, 2 * sms}) {
     char what[96]; snprintf(what, sizeof(what), "(d) shared-memory histogram, %d blocks x 1024 threads + flush", g);
     timeit(what, [&](bool prep) { if (!prep) k_hist_smem<<<g, 1024, nb * 4>>>(m, nb, hist); });
   }

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """Markdown summary of one `ncu --set full` capture, read back on the CPU box:
 
-   ncu -i gpurun_out/prof.ncu-rep --page raw --csv > /tmp/prof.csv
-   python tools/ncu_summary.py /tmp/prof.csv [kernel-substring] > profiles/rNN_ncu_<kernel>_summary.md
+   ncu -i prof.ncu-rep --page raw --csv > /tmp/prof.csv
+   python tools/ncu_summary.py /tmp/prof.csv [kernel-substring] > ncu_<kernel>_summary.md
 
 The CSV of `--page raw` has one row per profiled launch and one column per metric (first rows: names, then units).
 Only the metrics that matter on this path are kept: duration, the pipes (IMAD.WIDE issues on fmaheavy), issue rate,

@@ -8,8 +8,7 @@ known-discrete-log oracle for every configuration before it is timed):
 
 Knobs (read by the library at table upload / MSM time): GB200_MSM_WINDOW (window bits c), GB200_MSM_TASK_LEN,
 GB200_MSM_CHUNK, GB200_MSM_PRECOMP.  The cartesian product of all --set lists is run.  (Round 2 measured and removed the other round-1 knobs:
-hybrid / FP64-pipe accumulate, batched-affine levels, shared-memory accumulators, persistent grid -
-profiles/r02_ab_session.md.)
+hybrid / FP64-pipe accumulate, batched-affine levels, shared-memory accumulators, persistent grid - DESIGN.md §3.)
 """
 import argparse
 import itertools
