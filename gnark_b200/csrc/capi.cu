@@ -125,8 +125,15 @@ void msm_tuning(size_t n, int nwin, int c, int precomp, int acc_blocks_per_sm, u
     if (waste < best_waste - 0.005) { best_waste = waste; best = tl; }                 // ties: the longer task
     if (tl == lo) break;
   }
-  *task_len = (uint32_t)env_int("GB200_MSM_TASK_LEN", (int)best);
-  *chunk = (uint32_t)env_int("GB200_MSM_CHUNK", c >= 12 ? 8 : 4);
+  // Overrides (tools/sweep_msm.py).  Both are clamped here, the one place that fixes the plan, so that the workspace size
+  // and the run always agree.  A task length below 1 divides by zero on the host; above 2^30 the kernel's rounded-up
+  // task count (entries + task_len - 1, 32-bit) wraps and a bucket gets no task at all.  A chunk below 1 divides by zero;
+  // more than a set's 2^(c-1) buckets only leaves one chunk per set.  An override out of range keeps the default.
+  const int tl_env = env_int("GB200_MSM_TASK_LEN", 0);
+  *task_len = tl_env >= 1 ? (uint32_t)(tl_env < (1 << 30) ? tl_env : (1 << 30)) : (uint32_t)best;
+  const int ch_env = env_int("GB200_MSM_CHUNK", 0);
+  const uint32_t set_size = 1u << (c - 1);
+  *chunk = ch_env >= 1 ? ((uint32_t)ch_env < set_size ? (uint32_t)ch_env : set_size) : (c >= 12 ? 8u : 4u);
 }
 
 int32_t scratch_alloc(int dev, size_t bytes, void** out) {
