@@ -719,6 +719,36 @@ int32_t b200_ntt(b200_domain_t d, void* data, int32_t on_dev, int32_t inverse, i
   GUARD_END
 }
 
+// group-element NTT of the domain's size on G1 points of the domain's curve (points_ntt.cuh), host or device buffer
+int32_t b200_points_ntt(b200_domain_t d, int32_t group, void* points_affine, int32_t points_on_dev, int32_t inverse) {
+  GUARD_BEGIN
+  if (!d) return set_error("points_ntt: null domain");
+  if (!points_affine) return set_error("points_ntt: null points");
+  if (group != 1) return set_error("points_ntt: only G1 is supported (group must be 1; G2 is not supported)");
+  const MsmOps* ops = get_msm_ops(d->curve, group);
+  if (!ops || !ops->points_ntt) return set_error("points_ntt: unsupported curve");
+  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
+  rc = msm_join(ctx); if (rc) return rc;
+  const size_t bytes = ((size_t)1 << d->logn) * ops->affine_bytes;
+  void* buf = points_affine;
+  AsyncBuf tmp;
+  if (!points_on_dev) {
+    CK(tmp.alloc(bytes, ctx->stream));
+    buf = tmp.p;
+    CK(cudaMemcpyAsync(buf, points_affine, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  cudaError_t e = ops->points_ntt(ctx->stream, d->impl, buf, inverse);
+  if (!points_on_dev) {
+    if (e == cudaSuccess) e = cudaMemcpyAsync(points_affine, buf, bytes, cudaMemcpyDeviceToHost, ctx->stream);
+    tmp.release_on(ctx->stream);
+  }
+  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);   // host pointers are only borrowed for the call
+  if (e != cudaSuccess) return cuda_fail("points_ntt", e);
+  if (e2 != cudaSuccess) return cuda_fail("points_ntt", e2);
+  return 0;
+  GUARD_END
+}
+
 int32_t b200_groth16_compute_h(b200_domain_t d, const void* a, const void* b, const void* c, size_t len,
                                int32_t in_dev, void* h_out, int32_t out_dev) {
   GUARD_BEGIN

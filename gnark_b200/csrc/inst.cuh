@@ -7,6 +7,7 @@
 #include "msm_impl.cuh"
 #include "ntt_impl.cuh"
 #include "plonk.cuh"
+#include "points_ntt.cuh"
 #include "../../include/gnark_b200.h"
 
 namespace gb200 {
@@ -85,7 +86,17 @@ struct MsmInst {
   }
   static const MsmOps* ops() {
     static const MsmOps o = {Fr::Params::BITS, sizeof(Fr), sizeof(Affine<F>), sizeof(Jacobian<F>), &ws_bytes, &run,
-                             &precompute, &acc_blocks_per_sm, &fixed_base, &fold, &encoded_bytes, &decode};
+                             &precompute, &acc_blocks_per_sm, &fixed_base, &fold, &encoded_bytes, &decode, nullptr};
+    return &o;
+  }
+  // G1 only: the group NTT is instantiated through ops_g1(), so G2 compiles none of its kernels
+  static cudaError_t points_ntt(cudaStream_t st, void* dom, void* d_points, int inverse) {
+    const NttDomainDev<Fr>& d = *reinterpret_cast<const NttDomainDev<Fr>*>(dom);
+    return points_ntt_enqueue<Fr, F>(st, d.logn, inverse ? d.itw : d.tw, d.ninv, inverse != 0,
+                                     reinterpret_cast<Affine<F>*>(d_points));
+  }
+  static const MsmOps* ops_g1() {
+    static const MsmOps o = [] { MsmOps x = *ops(); x.points_ntt = &points_ntt; return x; }();
     return &o;
   }
 };
@@ -416,6 +427,12 @@ struct HostGroupInst {
   namespace {                                                                       \
   struct RegistrarMsm_##TAG {                                                       \
     RegistrarMsm_##TAG() { register_msm_ops(ID, GROUP, MsmInst<FR, F>::ops()); }    \
+  } registrar_msm_##TAG;                                                            \
+  }
+#define GB200_REGISTER_MSM_G1(TAG, ID, FR, F)                                     \
+  namespace {                                                                       \
+  struct RegistrarMsm_##TAG {                                                       \
+    RegistrarMsm_##TAG() { register_msm_ops(ID, 1, MsmInst<FR, F>::ops_g1()); }     \
   } registrar_msm_##TAG;                                                            \
   }
 #define GB200_REGISTER_FR(TAG, ID, FR, HFR, HFP, HG2F)                             \

@@ -64,6 +64,9 @@ struct MsmOps {
   size_t (*encoded_bytes)(int encoding);
   cudaError_t (*decode)(cudaStream_t st, const void* d_bytes, size_t n, int encoding, int curve, int group, void* d_out_affine,
                         uint32_t* d_status);
+  // group-element NTT (points_ntt.cuh) in place on the 2^logn device points of d_points, on the NttDomainDev of the same
+  // curve's Fr behind `dom`; G1 only (null for G2)
+  cudaError_t (*points_ntt)(cudaStream_t st, void* dom, void* d_points, int inverse);
 };
 
 struct NttOps {

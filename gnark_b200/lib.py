@@ -39,6 +39,7 @@ EXPORTS = [
     "b200_comm_unique_id", "b200_comm_init", "b200_comm_init_all", "b200_comm_destroy", "b200_comm_info",
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
+    "b200_points_ntt",
 ]
 COMM_ID_BYTES = 128
 
@@ -181,6 +182,8 @@ def load(path: str = None):
     lib.b200_ntt_domain_free.argtypes = [vp]
     lib.b200_ntt.argtypes = [vp, vp, i32, i32, i32, i32]
     lib.b200_ntt_async.argtypes = [vp, vp, i32, i32, i32]
+    if "b200_points_ntt" not in missing:
+        lib.b200_points_ntt.argtypes = [vp, i32, vp, i32, i32]
     lib.b200_groth16_compute_h.argtypes = [vp, vp, vp, vp, sz, i32, vp, i32]
     lib.b200_vec_op.argtypes = [i32, i32, i32, vp, vp, vp, sz]
     lib.b200_vec_bit_reverse.argtypes = [i32, i32, vp, u32]
@@ -446,6 +449,16 @@ class Domain:
 
     def ntt_async(self, d_data, inverse=False, decimation=DIF, on_coset=False):
         check(load().b200_ntt_async(self.handle, ptr(d_data), 1 if inverse else 0, decimation, 1 if on_coset else 0))
+
+    def points_ntt(self, points, group=1, inverse=True):
+        """Group-element NTT of 2^log2n affine points of this domain's curve (kzg.ToLagrangeG1 for inverse=True:
+        monomial SRS [tau^k]G -> Lagrange basis [L_i(tau)]G; inverse=False goes back), natural order in and out.
+        A numpy array is transformed in a copy that is returned; a device tensor in place (and returned)."""
+        on_dev = hasattr(points, "data_ptr")
+        if not on_dev:
+            points = np.array(points, dtype=np.uint64, order="C", copy=True)
+        check(load().b200_points_ntt(self.handle, group, ptr(points), 1 if on_dev else 0, 1 if inverse else 0))
+        return points
 
     def compute_h(self, a, b, c, length=None, on_device=False, out=None, out_on_device=False):
         if length is None:

@@ -296,3 +296,22 @@ func (s *PlonkSession) End() {
 		s.h = nil
 	}
 }
+
+// PointsNTT is b200_points_ntt on a domain of 2^log2n points created for the call with gnark-crypto's fft.NewDomain
+// generator: points (2^log2n G1Affine of `curve`, host memory, borrowed for the call) are transformed in place, natural
+// order in and out; inverse = monomial SRS -> Lagrange basis (kzg.ToLagrangeG1), otherwise back.
+func PointsNTT(dev int, curve int32, log2n uint32, points unsafe.Pointer, inverse bool) error {
+	var d C.b200_domain_t
+	err := Call(func() int32 {
+		return int32(C.b200_ntt_domain_new(C.int32_t(dev), C.int32_t(curve), C.uint32_t(log2n), nil, nil, &d))
+	})
+	if err != nil {
+		return err
+	}
+	defer C.b200_ntt_domain_free(d)
+	inv := C.int32_t(0)
+	if inverse {
+		inv = 1
+	}
+	return Call(func() int32 { return int32(C.b200_points_ntt(d, 1, points, 0, inv)) })
+}

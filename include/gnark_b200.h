@@ -219,6 +219,16 @@ int32_t b200_ntt_domain_free(b200_domain_t d);
 int32_t b200_ntt(b200_domain_t d, void* data, int32_t data_on_dev, int32_t inverse, int32_t decimation,
                  int32_t on_coset);
 int32_t b200_ntt_async(b200_domain_t d, void* d_data, int32_t inverse, int32_t decimation, int32_t on_coset);
+/* Group-element NTT: a KZG SRS between monomial form [tau^k]G and the Lagrange basis [L_i(tau)]G (SURVEY.md §8(f)-3).
+ * Replaces gnark-crypto's kzg.ToLagrangeG1 (as used at std/recursion/plonk/verifier_test.go:370; in-tree statement
+ * lagrangeCoeffsG1, backend/groth16/<curve>/mpcsetup/lagrange.go:21-41), the route of a ceremony SRS without a trapdoor;
+ * test/unsafekzg/kzgsrs.go:184 takes the trapdoor shortcut instead.  points_affine: 2^log2n G1Affine of the domain's
+ * curve, host or device, transformed in place with the domain's generator w (its coset is not used):
+ *   inverse = 1 (monomial -> Lagrange): out[i] = (1/n) sum_k w^(-ik) in[k]
+ *   inverse = 0 (Lagrange -> monomial): out[k] = sum_i w^(ik) in[i]
+ * Natural order in and out; results are canonical affine points ((0,0) = infinity); n = 1 leaves the input unchanged.
+ * Synchronous.  group must be 1: G2 is not supported. */
+int32_t b200_points_ntt(b200_domain_t d, int32_t group, void* points_affine, int32_t points_on_dev, int32_t inverse);
 
 /* ---- Groth16 quotient (replaces computeH icicle.go:1391-1488; CPU twin
  *      prove.go:346-389).  a,b,c: `len` fr.Elements each (len <= n, zero padded
