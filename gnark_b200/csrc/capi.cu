@@ -200,6 +200,75 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
   return 0;
 }
 
+Staging::~Staging() { for (void* p : bufs_) cudaFreeAsync(p, ctx_->stream); }
+
+cudaError_t Staging::scratch(size_t bytes, void** d) {
+  cudaError_t e = cudaMallocAsync(d, bytes ? bytes : 1, ctx_->stream);
+  if (e == cudaSuccess) bufs_.push_back(*d);
+  return e;
+}
+
+cudaError_t Staging::upload(void* d_dst, const void* src, size_t bytes, bool src_on_dev) {
+  return cudaMemcpyAsync(d_dst, src, bytes, src_on_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx_->stream);
+}
+
+void Staging::download(void* dst, const void* d_src, size_t bytes, bool dst_on_dev) {
+  downloads_.push_back({dst, d_src, bytes, dst_on_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost});
+}
+
+cudaError_t Staging::stage(void* p, size_t bytes, bool on_dev, bool up, bool down, void** d) {
+  *d = p;
+  if (on_dev || bytes == 0) return cudaSuccess;
+  cudaError_t e = scratch(bytes, d);
+  if (e == cudaSuccess && up) e = upload(*d, p, bytes, false);
+  if (e == cudaSuccess && down) download(p, *d, bytes, false);
+  return e;
+}
+
+int32_t Staging::finish(const char* what, int32_t rc, cudaError_t e) {
+  if (rc == 0 && e == cudaSuccess)
+    for (const Copy& c : downloads_)
+      if ((e = cudaMemcpyAsync(c.dst, c.src, c.bytes, c.kind, ctx_->stream)) != cudaSuccess) break;
+  for (void* p : bufs_) cudaFreeAsync(p, ctx_->stream);
+  bufs_.clear();
+  const cudaError_t e_sync = cudaStreamSynchronize(ctx_->stream);
+  if (rc) return rc;
+  if (e != cudaSuccess) return cuda_fail(what, e);
+  if (e_sync != cudaSuccess) return cuda_fail(what, e_sync);
+  return 0;
+}
+
+// b200_msm_submit / b200_msm_submit_dev: the scalars go up on the copy stream (overlapping the MSM before), the MSM is
+// pipelined; out_host == nullptr leaves the result in d_out, otherwise it is downloaded where the MSM produced it
+static int32_t msm_submit(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* scalars_host, void* d_out,
+                          void* out_host) {
+  AsyncBuf d_sc, out_buf;
+  if (out_host) {
+    CK(out_buf.alloc(t->ops->jac_bytes, ctx->stream));
+    d_out = out_buf.p;
+  }
+  if (n) {
+    CK(d_sc.alloc(n * t->ops->fr_bytes, ctx->copy_stream));
+    CK(cudaMemcpyAsync(d_sc.p, scalars_host, n * t->ops->fr_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+    CK(cudaEventRecord(ctx->copy_ev, ctx->copy_stream));
+    CK(cudaStreamWaitEvent(ctx->stream, ctx->copy_ev, 0));
+  }
+  int32_t rc = msm_on_stream(ctx, t, off, n, d_sc.p, d_out, nullptr, /*pipelined=*/true);
+  // the result is produced on the tail stream when the call was pipelined (n > 0), else on the main stream
+  cudaStream_t res_stream = (n > 0) ? ctx->tail_stream : ctx->stream;
+  if (rc == 0 && out_host) {
+    cudaError_t e = cudaMemcpyAsync(out_host, d_out, t->ops->jac_bytes, cudaMemcpyDeviceToHost, res_stream);
+    if (e != cudaSuccess) rc = cuda_fail("msm_submit result copy", e);
+    if (rc == 0 && n > 0) {   // the join point must cover the download too
+      e = cudaEventRecord(ctx->tail_ev, ctx->tail_stream);
+      if (e != cudaSuccess) rc = cuda_fail("cudaEventRecord", e);
+    }
+  }
+  d_sc.release_on(ctx->stream);       // last read by the decompose kernel on the main stream
+  out_buf.release_on(res_stream);
+  return rc;
+}
+
 }  // namespace gb200
 
 using namespace gb200;
@@ -222,7 +291,7 @@ int32_t b200_device_count(int32_t* out) {
 int32_t b200_init(int32_t n_dev, const int32_t* dev_ids) {
   GUARD_BEGIN
   if (n_dev <= 0 || !dev_ids) { DeviceCtx* c; return device_ctx(0, &c); }
-  for (int i = 0; i < n_dev; i++) { GB_DEVICE(c, dev_ids[i]); [[maybe_unused]] int32_t rc = 0; }
+  for (int i = 0; i < n_dev; i++) { GB_DEVICE(c, dev_ids[i]); }
   return 0;
   GUARD_END
 }
@@ -258,7 +327,7 @@ int32_t b200_shutdown(void) {
 
 int32_t b200_set_stream(int32_t dev, void* stream) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(c, dev);
   c->stream = stream ? reinterpret_cast<cudaStream_t>(stream) : c->own_stream;
   return 0;
   GUARD_END
@@ -266,8 +335,8 @@ int32_t b200_set_stream(int32_t dev, void* stream) {
 
 int32_t b200_sync(int32_t dev) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
-  rc = msm_join(c); if (rc) return rc;
+  GB_DEVICE(c, dev);
+  int32_t rc = msm_join(c); if (rc) return rc;
   CK(cudaStreamSynchronize(c->stream));
   return 0;
   GUARD_END
@@ -275,14 +344,14 @@ int32_t b200_sync(int32_t dev) {
 
 int32_t b200_alloc(int32_t dev, size_t bytes, void** out) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(c, dev);
   CK(cudaMalloc(out, bytes ? bytes : 1));
   return 0;
   GUARD_END
 }
 int32_t b200_free(int32_t dev, void* p) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(c, dev);
   CK(cudaStreamSynchronize(c->stream));
   CK(cudaFree(p));
   return 0;
@@ -290,7 +359,7 @@ int32_t b200_free(int32_t dev, void* p) {
 }
 int32_t b200_h2d(int32_t dev, void* dst, const void* src, size_t bytes) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(c, dev);
   CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, c->stream));
   CK(cudaStreamSynchronize(c->stream));  // host pointer is only borrowed for the call
   return 0;
@@ -298,8 +367,8 @@ int32_t b200_h2d(int32_t dev, void* dst, const void* src, size_t bytes) {
 }
 int32_t b200_d2h(int32_t dev, void* dst, const void* src, size_t bytes) {
   GUARD_BEGIN
-  GB_DEVICE(c, dev); [[maybe_unused]] int32_t rc = 0;
-  rc = msm_join(c); if (rc) return rc;
+  GB_DEVICE(c, dev);
+  int32_t rc = msm_join(c); if (rc) return rc;
   CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
@@ -352,11 +421,11 @@ extern "C" {
 int32_t b200_table_upload(int32_t dev, int32_t curve, int32_t group, const void* points, size_t n, int32_t flags,
                           b200_table_t* out) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   if (!out) return set_error("table_upload: null argument");
   if (n && !points) return set_error("table_upload: null points");
   std::unique_ptr<b200_table_s> t;
-  rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
+  int32_t rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
   const cudaMemcpyKind kind = (flags & B200_TABLE_SRC_ON_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   if (n) CK(cudaMemcpyAsync(t->d_points, points, n * t->ops->affine_bytes, kind, ctx->stream));
   rc = table_finish(ctx, t.get()); if (rc) return rc;
@@ -373,26 +442,27 @@ int32_t b200_table_upload(int32_t dev, int32_t curve, int32_t group, const void*
 int32_t b200_table_upload_encoded(int32_t dev, int32_t curve, int32_t group, const void* bytes, size_t n, int32_t encoding,
                                   int32_t flags, b200_table_t* out) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   if (!out || (n && !bytes)) return set_error("table_upload_encoded: null argument");
   if (flags & B200_TABLE_SRC_ON_DEVICE) return set_error("table_upload_encoded: the encoded slice is read from host memory");
   if (curve < 0 || curve > 3) return set_error("table_upload_encoded: unsupported curve");
   std::unique_ptr<b200_table_s> t;
-  rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
+  int32_t rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
   const size_t per = t->ops->encoded_bytes(encoding);
   if (per == 0) return set_error("table_upload_encoded: unknown encoding (1 = raw, 2 = compressed)");
   if (n) {
-    AsyncBuf d_bytes, d_status;
-    CK(d_bytes.alloc(n * per, ctx->stream));
-    CK(d_status.alloc(2 * sizeof(uint32_t), ctx->stream));
-    CK(cudaMemsetAsync(d_status.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-    CK(cudaMemcpyAsync(d_bytes.p, bytes, n * per, cudaMemcpyHostToDevice, ctx->stream));
-    cudaError_t e = t->ops->decode(ctx->stream, d_bytes.p, n, encoding, curve, group, t->d_points, (uint32_t*)d_status.p);
+    Staging st(ctx);
+    uint32_t status[2] = {0, 0};
+    const void* d_bytes;
+    void* d_status;
+    CK(st.in(bytes, n * per, false, &d_bytes));
+    CK(st.out(status, sizeof(status), false, &d_status));
+    CK(cudaMemsetAsync(d_status, 0, sizeof(status), ctx->stream));
+    cudaError_t e = t->ops->decode(ctx->stream, d_bytes, n, encoding, curve, group, t->d_points, (uint32_t*)d_status);
     if (e == cudaErrorNotSupported) return set_error("table_upload_encoded: encoding not supported for this group");
     if (e != cudaSuccess) return cuda_fail("points decode", e);
-    uint32_t status[2] = {0, 0};
-    CK(cudaMemcpyAsync(status, d_status.p, sizeof(status), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    rc = st.finish("table_upload_encoded", 0);
+    if (rc) return rc;
     if (status[0]) {
       static const char* why[] = {"", "invalid metadata bits", "coordinate not reduced modulo p", "point not on the curve"};
       return set_error(std::string("table_upload_encoded: point ") + std::to_string(status[1]) + ": " + why[status[0] < 4 ? status[0] : 0]);
@@ -415,7 +485,7 @@ int32_t b200_table_upload_file(int32_t dev, int32_t curve, int32_t group, const 
   GUARD_BEGIN
   if (!path || !out) return set_error("table_upload_file: null argument");
   if (flags & B200_TABLE_SRC_ON_DEVICE) return set_error("table_upload_file: the source is a file");
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const MsmOps* ops = get_msm_ops(curve, group);
   if (!ops) return set_error("table_upload_file: unsupported curve/group");
   const size_t bytes = n * ops->affine_bytes;
@@ -427,7 +497,7 @@ int32_t b200_table_upload_file(int32_t dev, int32_t curve, int32_t group, const 
   if ((uint64_t)st.st_size < byte_offset || (uint64_t)st.st_size - byte_offset < bytes)
     return set_error("table_upload_file: [offset, offset + n * sizeof(point)) exceeds the file");
   std::unique_ptr<b200_table_s> t;
-  rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
+  int32_t rc = table_new(dev, curve, group, n, flags, t); if (rc) return rc;
   if (n) {
     // the file region goes through two pinned slots straight into slab 0 of the table: no second device copy of the
     // slice, peak HBM = the table itself
@@ -470,7 +540,7 @@ int32_t b200_table_upload_file(int32_t dev, int32_t curve, int32_t group, const 
 int32_t b200_table_free(b200_table_t t) {
   GUARD_BEGIN
   if (!t) return 0;
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, t->dev);
   CK(cudaStreamSynchronize(ctx->stream));
   delete t;       // ~b200_table_s releases the device buffers
   return 0;
@@ -493,7 +563,7 @@ int32_t b200_table_info(b200_table_t t, size_t* n, int32_t* c, int32_t* nwin, in
 int32_t b200_msm_async(b200_table_t t, size_t off, size_t n, const void* d_scalars, void* d_out) {
   GUARD_BEGIN
   if (!t) return set_error("msm: null table");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, t->dev);
   return msm_on_stream(ctx, t, off, n, d_scalars, d_out);
   GUARD_END
 }
@@ -502,32 +572,20 @@ int32_t b200_fixed_base_batch(int32_t dev, int32_t curve, int32_t group, const v
                               const void* scalars, int32_t scalars_on_device, size_t n, void* out_affine,
                               int32_t out_on_device) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const MsmOps* ops = get_msm_ops(curve, group);
   if (!ops) return set_error("fixed_base_batch: unsupported curve/group");
   if (!base_affine || (n && (!scalars || !out_affine))) return set_error("fixed_base_batch: null argument");
   if (n == 0) return 0;
-  rc = msm_join(ctx); if (rc) return rc;
-  void* d_sc = const_cast<void*>(scalars);
-  void* d_out = out_affine;
-  AsyncBuf sc_buf, out_buf;
-  if (!scalars_on_device) {
-    CK(sc_buf.alloc(n * ops->fr_bytes, ctx->stream));
-    d_sc = sc_buf.p;
-    CK(cudaMemcpyAsync(d_sc, scalars, n * ops->fr_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  if (!out_on_device) { CK(out_buf.alloc(n * ops->affine_bytes, ctx->stream)); d_out = out_buf.p; }
+  int32_t rc = msm_join(ctx); if (rc) return rc;
+  Staging st(ctx);
+  const void* d_sc;
+  void* d_out;
+  CK(st.in(scalars, n * ops->fr_bytes, scalars_on_device, &d_sc));
+  CK(st.out(out_affine, n * ops->affine_bytes, out_on_device, &d_out));
   int c = env_int("GB200_FIXED_BASE_WINDOW", 0);
   if (c < 2 || c > 16) c = fixed_base_window_for(n);
-  cudaError_t e = ops->fixed_base(ctx->stream, base_affine, d_sc, n, c, d_out);
-  if (e == cudaSuccess && !out_on_device)
-    e = cudaMemcpyAsync(out_affine, d_out, n * ops->affine_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-  sc_buf.release_on(ctx->stream);
-  out_buf.release_on(ctx->stream);
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);   // host pointers are only borrowed for the call
-  if (e != cudaSuccess) return cuda_fail("fixed_base_batch", e);
-  if (e2 != cudaSuccess) return cuda_fail("fixed_base_batch", e2);
-  return 0;
+  return st.finish("fixed_base_batch", ops->fixed_base(ctx->stream, base_affine, d_sc, n, c, d_out));
   GUARD_END
 }
 
@@ -536,10 +594,10 @@ int32_t b200_fixed_base_batch(int32_t dev, int32_t curve, int32_t group, const v
 int32_t b200_msm_profile(b200_table_t t, size_t off, size_t n, const void* d_scalars, void* d_out, float* stage_ms) {
   GUARD_BEGIN
   if (!t || !stage_ms) return set_error("msm_profile: null argument");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, t->dev);
   cudaEvent_t ev[8];
   for (int k = 0; k < 8; k++) CK(cudaEventCreate(&ev[k]));
-  rc = msm_on_stream(ctx, t, off, n, d_scalars, d_out, ev);
+  int32_t rc = msm_on_stream(ctx, t, off, n, d_scalars, d_out, ev);
   cudaError_t e = cudaStreamSynchronize(ctx->stream);
   if (rc == 0 && e == cudaSuccess && n > 0)
     for (int k = 0; k < 7; k++) cudaEventElapsedTime(&stage_ms[k], ev[k], ev[k + 1]);
@@ -553,13 +611,13 @@ int32_t b200_msm_profile(b200_table_t t, size_t off, size_t n, const void* d_sca
 int32_t b200_msm_pipelined(b200_table_t t, size_t off, size_t n, const void* d_scalars, void* d_out) {
   GUARD_BEGIN
   if (!t) return set_error("msm: null table");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, t->dev);
   return msm_on_stream(ctx, t, off, n, d_scalars, d_out, nullptr, true);
   GUARD_END
 }
 int32_t b200_msm_join(int32_t dev) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   return msm_join(ctx);
   GUARD_END
 }
@@ -568,26 +626,13 @@ int32_t b200_msm(b200_table_t t, size_t off, size_t n, const void* scalars, int3
   GUARD_BEGIN
   if (!t) return set_error("msm: null table");
   if (n && !scalars) return set_error("msm: null scalars");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
-  AsyncBuf d_sc, d_out;      // released on every path, early error returns included
-  CK(d_out.alloc(t->ops->jac_bytes, ctx->stream));
-  const void* sc = scalars;
-  if (!on_dev && n) {
-    CK(d_sc.alloc(n * t->ops->fr_bytes, ctx->stream));
-    CK(cudaMemcpyAsync(d_sc.p, scalars, n * t->ops->fr_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    sc = d_sc.p;
-  }
-  rc = msm_on_stream(ctx, t, off, n, sc, d_out.p);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(out_host, d_out.p, t->ops->jac_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e != cudaSuccess) rc = cuda_fail("msm result copy", e);
-  }
-  d_sc.release_on(ctx->stream);
-  d_out.release_on(ctx->stream);
-  cudaError_t e = cudaStreamSynchronize(ctx->stream);
-  if (rc) return rc;
-  if (e != cudaSuccess) return cuda_fail("msm", e);
-  return 0;
+  GB_DEVICE(ctx, t->dev);
+  Staging st(ctx);
+  void* d_out;
+  const void* sc;
+  CK(st.out(out_host, t->ops->jac_bytes, false, &d_out));
+  CK(st.in(scalars, n * t->ops->fr_bytes, on_dev, &sc));
+  return st.finish("msm", msm_on_stream(ctx, t, off, n, sc, d_out));
   GUARD_END
 }
 
@@ -599,29 +644,8 @@ int32_t b200_msm_submit(b200_table_t t, size_t off, size_t n, const void* scalar
   GUARD_BEGIN
   if (!t) return set_error("msm_submit: null table");
   if (!out_host || (n && !scalars_host)) return set_error("msm_submit: null argument");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
-  AsyncBuf d_sc, d_out;
-  CK(d_out.alloc(t->ops->jac_bytes, ctx->stream));
-  if (n) {
-    CK(d_sc.alloc(n * t->ops->fr_bytes, ctx->copy_stream));
-    CK(cudaMemcpyAsync(d_sc.p, scalars_host, n * t->ops->fr_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
-    CK(cudaEventRecord(ctx->copy_ev, ctx->copy_stream));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->copy_ev, 0));
-  }
-  rc = msm_on_stream(ctx, t, off, n, d_sc.p, d_out.p, nullptr, /*pipelined=*/true);
-  // the result is produced on the tail stream when the call was pipelined (n > 0), else on the main stream
-  cudaStream_t res_stream = (n > 0) ? ctx->tail_stream : ctx->stream;
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(out_host, d_out.p, t->ops->jac_bytes, cudaMemcpyDeviceToHost, res_stream);
-    if (e != cudaSuccess) rc = cuda_fail("msm_submit result copy", e);
-    if (rc == 0 && n > 0) {   // the join point must cover the download too
-      e = cudaEventRecord(ctx->tail_ev, ctx->tail_stream);
-      if (e != cudaSuccess) rc = cuda_fail("cudaEventRecord", e);
-    }
-  }
-  d_sc.release_on(ctx->stream);       // last read by the decompose kernel on the main stream
-  d_out.release_on(res_stream);
-  return rc;
+  GB_DEVICE(ctx, t->dev);
+  return msm_submit(ctx, t, off, n, scalars_host, nullptr, out_host);
   GUARD_END
 }
 
@@ -631,17 +655,8 @@ int32_t b200_msm_submit_dev(b200_table_t t, size_t off, size_t n, const void* sc
   GUARD_BEGIN
   if (!t) return set_error("msm_submit_dev: null table");
   if (!d_out_jac || (n && !scalars_host)) return set_error("msm_submit_dev: null argument");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
-  AsyncBuf d_sc;
-  if (n) {
-    CK(d_sc.alloc(n * t->ops->fr_bytes, ctx->copy_stream));
-    CK(cudaMemcpyAsync(d_sc.p, scalars_host, n * t->ops->fr_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
-    CK(cudaEventRecord(ctx->copy_ev, ctx->copy_stream));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->copy_ev, 0));
-  }
-  rc = msm_on_stream(ctx, t, off, n, d_sc.p, d_out_jac, nullptr, /*pipelined=*/true);
-  d_sc.release_on(ctx->stream);       // last read by the decompose kernel on the main stream
-  return rc;
+  GB_DEVICE(ctx, t->dev);
+  return msm_submit(ctx, t, off, n, scalars_host, d_out_jac, nullptr);
   GUARD_END
 }
 
@@ -658,7 +673,7 @@ int32_t b200_msm_g2(b200_table_t t, size_t off, size_t n, const void* s, int32_t
 int32_t b200_ntt_domain_new(int32_t dev, int32_t curve, uint32_t log2n, const void* gen, const void* coset,
                             b200_domain_t* out) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("ntt_domain_new: unsupported curve");
   if ((int)log2n > ops->two_adicity || log2n > 30)
@@ -676,7 +691,7 @@ int32_t b200_ntt_domain_new(int32_t dev, int32_t curve, uint32_t log2n, const vo
 int32_t b200_ntt_domain_free(b200_domain_t d) {
   GUARD_BEGIN
   if (!d) return 0;
-  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d->dev);
   CK(cudaStreamSynchronize(ctx->stream));
   d->ops->domain_free(d->impl);
   delete d;
@@ -688,7 +703,7 @@ int32_t b200_ntt_async(b200_domain_t d, void* d_data, int32_t inverse, int32_t d
   GUARD_BEGIN
   if (!d) return set_error("ntt: null domain");
   if (decimation != B200_DIF && decimation != B200_DIT) return set_error("ntt: decimation must be DIF or DIT");
-  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d->dev);
   CK(d->ops->ntt(ctx->stream, d->impl, d_data, inverse, decimation, on_coset));
   return 0;
   GUARD_END
@@ -698,24 +713,11 @@ int32_t b200_ntt(b200_domain_t d, void* data, int32_t on_dev, int32_t inverse, i
   GUARD_BEGIN
   if (!d) return set_error("ntt: null domain");
   if (decimation != B200_DIF && decimation != B200_DIT) return set_error("ntt: decimation must be DIF or DIT");
-  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
-  const size_t bytes = ((size_t)1 << d->logn) * d->ops->fr_bytes;
-  void* buf = data;
-  AsyncBuf tmp;
-  if (!on_dev) {
-    CK(tmp.alloc(bytes, ctx->stream));
-    buf = tmp.p;
-    CK(cudaMemcpyAsync(buf, data, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  cudaError_t e = d->ops->ntt(ctx->stream, d->impl, buf, inverse, decimation, on_coset);
-  if (!on_dev) {
-    if (e == cudaSuccess) e = cudaMemcpyAsync(data, buf, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    tmp.release_on(ctx->stream);
-  }
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) return cuda_fail("ntt", e);
-  if (e2 != cudaSuccess) return cuda_fail("ntt", e2);
-  return 0;
+  GB_DEVICE(ctx, d->dev);
+  Staging st(ctx);
+  void* buf;
+  CK(st.inout(data, ((size_t)1 << d->logn) * d->ops->fr_bytes, on_dev, &buf));
+  return st.finish("ntt", d->ops->ntt(ctx->stream, d->impl, buf, inverse, decimation, on_coset));
   GUARD_END
 }
 
@@ -727,25 +729,12 @@ int32_t b200_points_ntt(b200_domain_t d, int32_t group, void* points_affine, int
   if (group != 1) return set_error("points_ntt: only G1 is supported (group must be 1; G2 is not supported)");
   const MsmOps* ops = get_msm_ops(d->curve, group);
   if (!ops || !ops->points_ntt) return set_error("points_ntt: unsupported curve");
-  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
-  rc = msm_join(ctx); if (rc) return rc;
-  const size_t bytes = ((size_t)1 << d->logn) * ops->affine_bytes;
-  void* buf = points_affine;
-  AsyncBuf tmp;
-  if (!points_on_dev) {
-    CK(tmp.alloc(bytes, ctx->stream));
-    buf = tmp.p;
-    CK(cudaMemcpyAsync(buf, points_affine, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  cudaError_t e = ops->points_ntt(ctx->stream, d->impl, buf, inverse);
-  if (!points_on_dev) {
-    if (e == cudaSuccess) e = cudaMemcpyAsync(points_affine, buf, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    tmp.release_on(ctx->stream);
-  }
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);   // host pointers are only borrowed for the call
-  if (e != cudaSuccess) return cuda_fail("points_ntt", e);
-  if (e2 != cudaSuccess) return cuda_fail("points_ntt", e2);
-  return 0;
+  GB_DEVICE(ctx, d->dev);
+  int32_t rc = msm_join(ctx); if (rc) return rc;
+  Staging st(ctx);
+  void* buf;
+  CK(st.inout(points_affine, ((size_t)1 << d->logn) * ops->affine_bytes, points_on_dev, &buf));
+  return st.finish("points_ntt", ops->points_ntt(ctx->stream, d->impl, buf, inverse));
   GUARD_END
 }
 
@@ -753,35 +742,28 @@ int32_t b200_groth16_compute_h(b200_domain_t d, const void* a, const void* b, co
                                int32_t in_dev, void* h_out, int32_t out_dev) {
   GUARD_BEGIN
   if (!d) return set_error("compute_h: null domain");
-  GB_DEVICE(ctx, d->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d->dev);
   const size_t n = (size_t)1 << d->logn;
   if (len > n) return set_error("compute_h: len exceeds the domain");
   const size_t fb = d->ops->fr_bytes;
-  AsyncBuf vb[3];
-  void* v[3] = {nullptr, nullptr, nullptr};
+  // the transform works in place: device inputs are copied too, into buffers zero-padded to the domain
+  Staging st(ctx);
+  void* v[3];
   const void* src[3] = {a, b, c};
-  const cudaMemcpyKind kind = in_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   for (int k = 0; k < 3; k++) {
-    CK(vb[k].alloc(n * fb, ctx->stream));
-    v[k] = vb[k].p;
-    if (len) CK(cudaMemcpyAsync(v[k], src[k], len * fb, kind, ctx->stream));
+    CK(st.scratch(n * fb, &v[k]));
+    if (len) CK(st.upload(v[k], src[k], len * fb, in_dev));
     if (len < n) CK(cudaMemsetAsync((char*)v[k] + len * fb, 0, (n - len) * fb, ctx->stream));
   }
-  cudaError_t e = d->ops->compute_h(ctx->stream, d->impl, v[0], v[1], v[2]);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(h_out, v[0], n * fb, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream);
-  for (int k = 0; k < 3; k++) vb[k].release_on(ctx->stream);
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) return cuda_fail("compute_h", e);
-  if (e2 != cudaSuccess) return cuda_fail("compute_h", e2);
-  return 0;
+  st.download(h_out, v[0], n * fb, out_dev);
+  return st.finish("compute_h", d->ops->compute_h(ctx->stream, d->impl, v[0], v[1], v[2]));
   GUARD_END
 }
 
 // ---- vector ops -----------------------------------------------------------------
 int32_t b200_vec_op(int32_t dev, int32_t curve, int32_t op, void* out, const void* a, const void* b, size_t n) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_op: unsupported curve");
   if (op < 0 || op > 2) return set_error("vec_op: unknown op");
@@ -791,7 +773,7 @@ int32_t b200_vec_op(int32_t dev, int32_t curve, int32_t op, void* out, const voi
 }
 int32_t b200_vec_bit_reverse(int32_t dev, int32_t curve, void* data, uint32_t log2n) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_bit_reverse: unsupported curve");
   CK(ops->bit_reverse(ctx->stream, data, log2n));
@@ -800,7 +782,7 @@ int32_t b200_vec_bit_reverse(int32_t dev, int32_t curve, void* data, uint32_t lo
 }
 int32_t b200_vec_scale_powers(int32_t dev, int32_t curve, void* data, size_t n, const void* s, const void* g) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_scale_powers: unsupported curve");
   CK(ops->scale_powers(ctx->stream, data, n, s, g));
@@ -810,7 +792,7 @@ int32_t b200_vec_scale_powers(int32_t dev, int32_t curve, void* data, size_t n, 
 
 int32_t b200_vec_batch_invert(int32_t dev, int32_t curve, void* data, size_t n) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_batch_invert: unsupported curve");
   CK(ops->batch_invert(ctx->stream, data, n));
@@ -820,7 +802,7 @@ int32_t b200_vec_batch_invert(int32_t dev, int32_t curve, void* data, size_t n) 
 
 int32_t b200_vec_axpy(int32_t dev, int32_t curve, void* y, const void* a, const void* x, size_t n) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_axpy: unsupported curve");
   if (!a || (n && (!y || !x))) return set_error("vec_axpy: null argument");
@@ -830,7 +812,7 @@ int32_t b200_vec_axpy(int32_t dev, int32_t curve, void* y, const void* a, const 
 }
 int32_t b200_vec_scan(int32_t dev, int32_t curve, int32_t op, void* data, size_t n, int32_t exclusive) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("vec_scan: unsupported curve");
   if (op != B200_SCAN_PRODUCT && op != B200_SCAN_SUM) return set_error("vec_scan: unknown op");
@@ -842,14 +824,14 @@ int32_t b200_plonk_build_z(b200_domain_t d0, const void* l, const void* r, const
                            const void* beta, const void* gamma, void* z) {
   GUARD_BEGIN
   if (!d0 || !l || !r || !o || !perm || !beta || !gamma || !z) return set_error("plonk_build_z: null argument");
-  GB_DEVICE(ctx, d0->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d0->dev);
   CK(d0->ops->plonk_build_z(ctx->stream, d0->impl, l, r, o, perm, beta, gamma, z));
   return 0;
   GUARD_END
 }
 int32_t b200_poly_eval(int32_t dev, int32_t curve, const void* c, size_t n, const void* x, void* out) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("poly_eval: unsupported curve");
   if (!x || !out || (n && !c)) return set_error("poly_eval: null argument");
@@ -859,7 +841,7 @@ int32_t b200_poly_eval(int32_t dev, int32_t curve, const void* c, size_t n, cons
 }
 int32_t b200_poly_div_by_linear(int32_t dev, int32_t curve, void* c, size_t n, const void* z, void* rem) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("poly_div_by_linear: unsupported curve");
   if (!z || !rem || (n && !c)) return set_error("poly_div_by_linear: null argument");
@@ -873,7 +855,7 @@ int32_t b200_plonk_constraints_coset(b200_domain_t d0, const void* big_coset_gen
                                      const b200_plonk_coset_args* args) {
   GUARD_BEGIN
   if (!d0 || !big_coset_gen || !big_gen || !args) return set_error("plonk_constraints_coset: null argument");
-  GB_DEVICE(ctx, d0->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d0->dev);
   cudaError_t e = d0->ops->plonk_coset(ctx->stream, d0->impl, big_coset_gen, big_gen, args);
   if (e == cudaErrorInvalidValue) return set_error("plonk_constraints_coset: invalid rho / coset index / blinding length");
   if (e != cudaSuccess) return cuda_fail("plonk_constraints_coset", e);
@@ -884,7 +866,7 @@ int32_t b200_plonk_bsb22_coset(b200_domain_t d0, const void* d_qcp, const void* 
                                void* d_out) {
   GUARD_BEGIN
   if (!d0 || !d_qcp || !d_pi2 || !d_out) return set_error("plonk_bsb22_coset: null argument");
-  GB_DEVICE(ctx, d0->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d0->dev);
   cudaError_t e = d0->ops->plonk_bsb22(ctx->stream, d0->impl, d_qcp, d_pi2, coset_index, rho, d_out);
   if (e == cudaErrorInvalidValue) return set_error("plonk_bsb22_coset: invalid rho / coset index");
   if (e != cudaSuccess) return cuda_fail("plonk_bsb22_coset", e);
@@ -894,7 +876,7 @@ int32_t b200_plonk_bsb22_coset(b200_domain_t d0, const void* d_qcp, const void* 
 int32_t b200_plonk_divide_by_zh(b200_domain_t d1, uint32_t log_n0, void* d_data) {
   GUARD_BEGIN
   if (!d1 || !d_data) return set_error("plonk_divide_by_zh: null argument");
-  GB_DEVICE(ctx, d1->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, d1->dev);
   cudaError_t e = d1->ops->plonk_divide_by_zh(ctx->stream, d1->impl, log_n0, d_data);
   if (e == cudaErrorInvalidValue) return set_error("plonk_divide_by_zh: invalid domain ratio");
   if (e != cudaSuccess) return cuda_fail("plonk_divide_by_zh", e);

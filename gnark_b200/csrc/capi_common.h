@@ -80,6 +80,41 @@ int32_t scratch_free(int dev, void* p);
 int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* d_scalars, void* d_out,
                       cudaEvent_t* stage_events = nullptr, bool pipelined = false);
 int32_t msm_join(DeviceCtx* ctx);  // make ctx->stream wait for the pipelined tails
+
+// Buffers of one synchronous entry point, all on ctx->stream.  Host pointers are borrowed for the call only: host
+// inputs are uploaded into pool buffers now, host outputs are downloaded by finish(), which also frees every buffer
+// (before the sync, so that the pool can reuse them) and synchronises - nothing is read after the call returns.
+// Device-resident and zero-byte buffers are used in place.  An early return frees the buffers without a sync.
+class Staging {
+ public:
+  explicit Staging(DeviceCtx* ctx) : ctx_(ctx) {}
+  ~Staging();
+  Staging(const Staging&) = delete;
+  Staging& operator=(const Staging&) = delete;
+
+  // *d = the device copy of src (read by the operation), of dst (written by it) or of p (both)
+  cudaError_t in(const void* src, size_t bytes, bool on_dev, const void** d) {
+    return stage(const_cast<void*>(src), bytes, on_dev, true, false, const_cast<void**>(d));
+  }
+  cudaError_t out(void* dst, size_t bytes, bool on_dev, void** d) { return stage(dst, bytes, on_dev, false, true, d); }
+  cudaError_t inout(void* p, size_t bytes, bool on_dev, void** d) { return stage(p, bytes, on_dev, true, true, d); }
+  cudaError_t scratch(size_t bytes, void** d);
+  // copy src (device or host) into the device buffer d_dst now
+  cudaError_t upload(void* d_dst, const void* src, size_t bytes, bool src_on_dev);
+  // copy the device buffer d_src to dst (device or host) in finish(), once the operation has succeeded
+  void download(void* dst, const void* d_src, size_t bytes, bool dst_on_dev);
+  // downloads (when rc == 0 and e == cudaSuccess), frees, synchronises; returns the first error of: rc, e, a
+  // download, the sync.  `what` labels the CUDA failures.
+  int32_t finish(const char* what, int32_t rc, cudaError_t e = cudaSuccess);
+  int32_t finish(const char* what, cudaError_t e) { return finish(what, 0, e); }
+
+ private:
+  struct Copy { void* dst; const void* src; size_t bytes; cudaMemcpyKind kind; };
+  cudaError_t stage(void* p, size_t bytes, bool on_dev, bool up, bool down, void** d);
+  DeviceCtx* ctx_;
+  std::vector<void*> bufs_;
+  std::vector<Copy> downloads_;
+};
 }
 
 #define CK(x)                                                        \

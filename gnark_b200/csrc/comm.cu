@@ -114,7 +114,7 @@ int32_t b200_comm_unique_id(void* out_id128) {
 int32_t b200_comm_init(int32_t dev, int32_t world, int32_t rank, const void* id128) {
   GUARD_BEGIN
   if (world < 1 || rank < 0 || rank >= world) return set_error("comm_init: need 0 <= rank < world");
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   comm_teardown(*ctx);
   if (world == 1) return 0;
   if (!id128) return set_error("comm_init: null unique id");
@@ -160,9 +160,9 @@ int32_t b200_comm_init_all(int32_t n_dev, const int32_t* dev_ids) {
 
 int32_t b200_comm_destroy(int32_t dev) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   if (ctx->comm) {
-    rc = msm_join(ctx); if (rc) return rc;
+    int32_t rc = msm_join(ctx); if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
   }
   comm_teardown(*ctx);
@@ -172,7 +172,7 @@ int32_t b200_comm_destroy(int32_t dev) {
 
 int32_t b200_comm_info(int32_t dev, int32_t* world, int32_t* rank) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   if (world) *world = ctx->comm ? ctx->comm_world : 1;
   if (rank) *rank = ctx->comm ? ctx->comm_rank : 0;
   return 0;
@@ -182,7 +182,7 @@ int32_t b200_comm_info(int32_t dev, int32_t* world, int32_t* rank) {
 int32_t b200_points_allreduce(int32_t dev, int32_t curve, int32_t group, const void* d_partials, size_t count,
                               void* d_totals) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const MsmOps* ops = get_msm_ops(curve, group);
   if (!ops) return set_error("points_allreduce: unsupported curve/group");
   if (count && (!d_partials || !d_totals)) return set_error("points_allreduce: null argument");
@@ -195,12 +195,12 @@ int32_t b200_points_allreduce(int32_t dev, int32_t curve, int32_t group, const v
 int32_t b200_points_fold(int32_t dev, int32_t curve, int32_t group, const void* d_gathered, uint32_t world, uint32_t count,
                          void* d_totals) {
   GUARD_BEGIN
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const MsmOps* ops = get_msm_ops(curve, group);
   if (!ops) return set_error("points_fold: unsupported curve/group");
   if (count && world && (!d_gathered || !d_totals)) return set_error("points_fold: null argument");
   if (world == 0) return set_error("points_fold: world must be at least 1");
-  rc = msm_join(ctx); if (rc) return rc;
+  int32_t rc = msm_join(ctx); if (rc) return rc;
   CK(ops->fold(ctx->stream, d_gathered, world, count, d_totals));
   return 0;
   GUARD_END
@@ -212,27 +212,15 @@ int32_t b200_msm_allreduce(b200_table_t t, size_t off, size_t n, const void* sca
   GUARD_BEGIN
   if (!t) return set_error("msm_allreduce: null table");
   if (!out_host || (n && !scalars)) return set_error("msm_allreduce: null argument");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
-  AsyncBuf d_sc, d_out;
-  CK(d_out.alloc(t->ops->jac_bytes, ctx->stream));
-  const void* sc = scalars;
-  if (!on_dev && n) {
-    CK(d_sc.alloc(n * t->ops->fr_bytes, ctx->stream));
-    CK(cudaMemcpyAsync(d_sc.p, scalars, n * t->ops->fr_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    sc = d_sc.p;
-  }
-  rc = msm_on_stream(ctx, t, off, n, sc, d_out.p);
-  if (rc == 0) rc = points_allreduce_on_stream(ctx, t->ops, d_out.p, 1, d_out.p);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(out_host, d_out.p, t->ops->jac_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e != cudaSuccess) rc = cuda_fail("msm_allreduce result copy", e);
-  }
-  d_sc.release_on(ctx->stream);
-  d_out.release_on(ctx->stream);
-  cudaError_t e = cudaStreamSynchronize(ctx->stream);
-  if (rc) return rc;
-  if (e != cudaSuccess) return cuda_fail("msm_allreduce", e);
-  return 0;
+  GB_DEVICE(ctx, t->dev);
+  Staging st(ctx);
+  void* d_out;
+  const void* sc;
+  CK(st.out(out_host, t->ops->jac_bytes, false, &d_out));
+  CK(st.in(scalars, n * t->ops->fr_bytes, on_dev, &sc));
+  int32_t rc = msm_on_stream(ctx, t, off, n, sc, d_out);
+  if (rc == 0) rc = points_allreduce_on_stream(ctx, t->ops, d_out, 1, d_out);
+  return st.finish("msm_allreduce", rc);
   GUARD_END
 }
 

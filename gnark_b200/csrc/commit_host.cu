@@ -61,30 +61,23 @@ int32_t b200_pedersen_commit(b200_pedersen_key_t key, const void* values, size_t
                                     " points (pedersen.ProvingKey.Commit requires equal lengths)");
   if (n && !values) return set_error("pedersen_commit: null values");
   if (!out_commitment && !out_pok) return 0;
-  GB_DEVICE(ctx, key->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, key->dev);
   const MsmOps* ops = key->basis->ops;
   const HostGroupOps* h = get_host_group_ops(key->curve, 1);
-  AsyncBuf d_sc, d_res;
-  CK(d_res.alloc(2 * ops->jac_bytes, ctx->stream));
-  const void* sc = values;
-  if (!values_on_device && n) {
-    CK(d_sc.alloc(n * ops->fr_bytes, ctx->stream));
-    CK(cudaMemcpyAsync(d_sc.p, values, n * ops->fr_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    sc = d_sc.p;
-  }
-  char* res = reinterpret_cast<char*>(d_res.p);
+  std::vector<uint8_t> host(2 * ops->jac_bytes);
+  Staging st(ctx);
+  void* d_res;
+  const void* sc;
+  CK(st.out(host.data(), host.size(), false, &d_res));
+  CK(st.in(values, n * ops->fr_bytes, values_on_device, &sc));
+  char* res = reinterpret_cast<char*>(d_res);
+  int32_t rc = 0;
   if (out_commitment) rc = msm_on_stream(ctx, key->basis, 0, n, sc, res, nullptr, true);
   if (!rc && out_pok) rc = msm_on_stream(ctx, key->basis_sigma, 0, n, sc, res + ops->jac_bytes, nullptr, true);
   if (!rc) rc = msm_join(ctx);
-  std::vector<uint8_t> host(2 * ops->jac_bytes);
-  cudaError_t e = cudaSuccess;
-  if (!rc) e = cudaMemcpyAsync(host.data(), d_res.p, host.size(), cudaMemcpyDeviceToHost, ctx->stream);
-  d_sc.release_on(ctx->stream);
-  d_res.release_on(ctx->stream);
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);    // host pointers are only borrowed for the call
+  rc = st.finish("pedersen_commit", rc);
   if (rc) return rc;
-  if (e != cudaSuccess) return cuda_fail("pedersen_commit", e);
-  if (e2 != cudaSuccess) return cuda_fail("pedersen_commit", e2);
+  // affine on the host, after the sync
   if (out_commitment) h->to_affine(host.data(), out_commitment);
   if (out_pok) h->to_affine(host.data() + ops->jac_bytes, out_pok);
   return 0;
@@ -125,38 +118,22 @@ int32_t b200_msm_gather(b200_table_t t, size_t off, const uint32_t* idx, size_t 
   GUARD_BEGIN
   if (!t) return set_error("msm_gather: null table");
   if (!out_jac_host || (n_idx && (!idx || !scalars))) return set_error("msm_gather: null argument");
-  GB_DEVICE(ctx, t->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, t->dev);
   const NttOps* fr = get_ntt_ops(t->curve);
   if (!fr) return set_error("msm_gather: unsupported curve");
   if (!idx_on_device)
     for (size_t j = 0; j < n_idx; j++)
       if (idx[j] >= n_scalars) return set_error("msm_gather: index " + std::to_string(idx[j]) + " out of range at position " + std::to_string(j));
   const size_t fb = t->ops->fr_bytes;
-  AsyncBuf d_sc, d_idx, d_g, d_out;
-  CK(d_out.alloc(t->ops->jac_bytes, ctx->stream));
-  const void* sc = scalars;
-  const uint32_t* ix = idx;
-  if (!scalars_on_device && n_scalars) {
-    CK(d_sc.alloc(n_scalars * fb, ctx->stream));
-    CK(cudaMemcpyAsync(d_sc.p, scalars, n_scalars * fb, cudaMemcpyHostToDevice, ctx->stream));
-    sc = d_sc.p;
-  }
-  if (!idx_on_device && n_idx) {
-    CK(d_idx.alloc(n_idx * sizeof(uint32_t), ctx->stream));
-    CK(cudaMemcpyAsync(d_idx.p, idx, n_idx * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    ix = reinterpret_cast<const uint32_t*>(d_idx.p);
-  }
-  CK(d_g.alloc(n_idx * fb, ctx->stream));
-  if (n_idx) CK(fr->gather(ctx->stream, d_g.p, sc, ix, n_idx));
-  rc = msm_on_stream(ctx, t, off, n_idx, d_g.p, d_out.p);
-  cudaError_t e = cudaSuccess;
-  if (!rc) e = cudaMemcpyAsync(out_jac_host, d_out.p, t->ops->jac_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-  d_sc.release_on(ctx->stream); d_idx.release_on(ctx->stream); d_g.release_on(ctx->stream); d_out.release_on(ctx->stream);
-  cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
-  if (rc) return rc;
-  if (e != cudaSuccess) return cuda_fail("msm_gather", e);
-  if (e2 != cudaSuccess) return cuda_fail("msm_gather", e2);
-  return 0;
+  Staging st(ctx);
+  void *d_out, *d_g;
+  const void *sc, *ix;
+  CK(st.out(out_jac_host, t->ops->jac_bytes, false, &d_out));
+  CK(st.in(scalars, n_scalars * fb, scalars_on_device, &sc));
+  CK(st.in(idx, n_idx * sizeof(uint32_t), idx_on_device, &ix));
+  CK(st.scratch(n_idx * fb, &d_g));
+  if (n_idx) CK(fr->gather(ctx->stream, d_g, sc, static_cast<const uint32_t*>(ix), n_idx));
+  return st.finish("msm_gather", msm_on_stream(ctx, t, off, n_idx, d_g, d_out));
   GUARD_END
 }
 

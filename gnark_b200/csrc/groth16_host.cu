@@ -62,7 +62,7 @@ int32_t b200_groth16_pk_free(b200_pk_t pk);
 int32_t b200_groth16_pk_load(int32_t dev, const b200_groth16_pk_desc* d, b200_pk_t* out) {
   GUARD_BEGIN
   if (!d || !out) return set_error("pk_load: null argument");
-  GB_DEVICE(ctx, dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, dev);
   const HostGroupOps* h1 = get_host_group_ops(d->curve, 1);
   const HostGroupOps* h2 = get_host_group_ops(d->curve, 2);
   const NttOps* fr = get_ntt_ops(d->curve);
@@ -160,7 +160,7 @@ int32_t b200_groth16_pk_load(int32_t dev, const b200_groth16_pk_desc* d, b200_pk
 int32_t b200_groth16_pk_free(b200_pk_t pk) {
   GUARD_BEGIN
   if (!pk) return 0;
-  GB_DEVICE(ctx, pk->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, pk->dev);
   cudaStreamSynchronize(ctx->stream);
   b200_table_free(pk->A); b200_table_free(pk->B1); b200_table_free(pk->Z); b200_table_free(pk->K); b200_table_free(pk->B2);
   b200_ntt_domain_free(pk->dom);
@@ -236,7 +236,7 @@ int32_t b200_groth16_msms(b200_pk_t pk, const void* wires, const void* a, const 
   if (!pk) return set_error("prove: null proving key");
   if (!wires || !a || !b || !c || !msm_out) return set_error("prove: null argument");
   if (n_constraints > pk->n) return set_error("prove: more constraints than the domain holds");
-  GB_DEVICE(ctx, pk->dev); [[maybe_unused]] int32_t rc = 0;
+  GB_DEVICE(ctx, pk->dev);
   cudaStream_t st = ctx->stream;
   const size_t fb = pk->fr->fr_bytes;
   const size_t n = pk->n;
@@ -272,7 +272,7 @@ int32_t b200_groth16_msms(b200_pk_t pk, const void* wires, const void* a, const 
   // wire filtering (prove.go:147-168) and the three MSMs that do not need h start right after W lands
   CK(pk->fr->gather(st, d_wa, d_w, pk->d_idx_a, pk->n_a));
   CK(pk->fr->gather(st, d_wb, d_w, pk->d_idx_b, pk->n_b));
-  rc = lap("h2d W+filter"); if (rc) return rc;
+  int32_t rc = lap("h2d W+filter"); if (rc) return rc;
   char* res = reinterpret_cast<char*>(d_res);
   // prove.go:207 (Ar), :194 (Bs1), :237 (Krs), :283 (Bs2), :227 (Krs2 over h)
   rc = msm_on_stream(ctx, pk->A, 0, pk->n_a, d_wa, res + 0 * j1, nullptr, true); if (rc) return rc;
