@@ -21,35 +21,16 @@
 
 using namespace gb200;
 
-struct b200_plonk_pk_s {
-  int dev = 0, curve = 0;
-  uint32_t logn = 0;
-  size_t n = 0;
-  size_t fb = 0;                      // sizeof(fr.Element)
-  const HostFrCtx* fr = nullptr;
-  HostFr g, w, w4;                    // FrMultiplicativeGen, domain0 generator, domain1 generator (Montgomery)
-  b200_domain_t dom0[4] = {nullptr, nullptr, nullptr, nullptr};   // domain0 with coset generator g * w4^i
-  b200_domain_t dom1 = nullptr;
-  // ql, qr, qm, qo, qk, s1, s2, s3
-  void* br[8] = {nullptr};            // canonical coefficients, bit-reversed layout (inputs of the coset NTTs)
-  void* canon[8] = {nullptr};         // canonical coefficients, regular layout
-  int64_t* d_perm = nullptr;
-  b200_table_t srs = nullptr;         // canonical SRS, n + 3 points
-  // BSB22 commitment gates: selectors Qcp_j (trace.Qcp), canonical bit-reversed / regular like the other key polys
-  std::vector<void*> qcp_br, qcp_canon;
-  // The key polynomials never change between proofs: their evaluations on the four cosets of the quotient domain
-  // are computed once at key load and kept in HBM ((8 + n_qcp) x 4 x n elements: 4 GiB at n = 2^22 with 32-byte
-  // elements), so a proof runs 16 coset NTTs (l, r, o, z) instead of 48.  key_cos[i][k]: coset i, polynomial k in the
-  // order ql qr qm qo qk s1 s2 s3 qcp...; empty when GB200_PLONK_COSET_CACHE=0.
-  std::vector<std::vector<void*>> key_cos;
-  // wall-clock ms of the five stages of the last b200_plonk_prove on this key (every stage ends in a b200_sync, so
-  // these are device times + host orchestration): begin (L,R,O), commit_z, quotient, linearise, batch_open
-  double last_stage_ms[5] = {0, 0, 0, 0, 0};
-};
-
 namespace gb200_plonk {
 
-enum { QL = 0, QR, QM, QO, QK, S1, S2, S3 };
+// index of a key polynomial: the fixed ones, then the BSB22 selectors Qcp_j (trace.Qcp) at QCP0 + j
+enum { QL = 0, QR, QM, QO, QK, S1, S2, S3, QCP0 };
+
+// a key polynomial's canonical coefficients, in the two layouts the prover reads
+struct KeyPoly {
+  void* br = nullptr;                 // bit-reversed (input of the coset NTTs)
+  void* canon = nullptr;              // regular
+};
 
 #define RC(x)                        \
   do {                               \
@@ -72,6 +53,29 @@ struct Scratch {
 
 }  // namespace gb200_plonk
 using namespace gb200_plonk;
+
+struct b200_plonk_pk_s {
+  int dev = 0, curve = 0;
+  uint32_t logn = 0;
+  size_t n = 0;
+  size_t fb = 0;                      // sizeof(fr.Element)
+  const HostFrCtx* fr = nullptr;
+  HostFr g, w, w4;                    // FrMultiplicativeGen, domain0 generator, domain1 generator (Montgomery)
+  b200_domain_t dom0[4] = {nullptr, nullptr, nullptr, nullptr};   // domain0 with coset generator g * w4^i
+  b200_domain_t dom1 = nullptr;
+  uint32_t n_qcp = 0;                 // BSB22 commitment gates
+  std::vector<KeyPoly> key;           // QCP0 + n_qcp polynomials, by the index above
+  int64_t* d_perm = nullptr;
+  b200_table_t srs = nullptr;         // canonical SRS, n + 3 points
+  // The key polynomials never change between proofs: their evaluations on the four cosets of the quotient domain
+  // are computed once at key load and kept in HBM ((8 + n_qcp) x 4 x n elements: 4 GiB at n = 2^22 with 32-byte
+  // elements), so a proof runs 16 coset NTTs (l, r, o, z) instead of 48.  key_cos[i][k]: coset i, key polynomial k;
+  // empty when GB200_PLONK_COSET_CACHE=0.
+  std::vector<std::vector<void*>> key_cos;
+  // wall-clock ms of the five stages of the last b200_plonk_prove on this key (every stage ends in a b200_sync, so
+  // these are device times + host orchestration): begin (L,R,O), commit_z, quotient, linearise, batch_open
+  double last_stage_ms[5] = {0, 0, 0, 0, 0};
+};
 
 // one proof in flight: what the later Fiat-Shamir rounds need from the earlier ones
 struct b200_plonk_session_s {
@@ -110,14 +114,27 @@ int32_t dzero(int dev, void* dst, size_t bytes) {
   return 0;
 }
 
+// Lagrange/regular values (n elements, on the host or the device) -> cb: canonical, bit-reversed ; reg: canonical,
+// regular (its first n elements)
+int32_t to_canonical(b200_plonk_pk_s* pk, const void* lagrange, bool on_host, void* cb, void* reg) {
+  const size_t bytes = pk->n * pk->fb;
+  RC(on_host ? b200_h2d(pk->dev, cb, lagrange, bytes) : d2d(pk->dev, cb, lagrange, bytes));
+  RC(b200_ntt_async(pk->dom0[0], cb, 1, B200_DIF, 0));
+  RC(d2d(pk->dev, reg, cb, bytes));
+  return b200_vec_bit_reverse(pk->dev, pk->curve, reg, pk->logn);
+}
+
+// canonical, bit-reversed (n elements) -> dst: values on coset i of the quotient domain, regular
+int32_t to_coset(b200_plonk_pk_s* pk, uint32_t i, const void* cb, void* dst) {
+  RC(d2d(pk->dev, dst, cb, pk->n * pk->fb));
+  return b200_ntt_async(pk->dom0[i], dst, 0, B200_DIT, 1);
+}
+
 // Lagrange/regular values (device, n elements) -> cb: canonical, bit-reversed (n) ; reg: canonical, regular,
 // blinded p + b(X)(X^n - 1) with nb blinding coefficients (n + nb elements)     (getBlindedCoefficients :1211-1220)
 int32_t canonical_blinded(b200_plonk_pk_s* pk, const void* d_lagrange, const uint8_t* b_mont, int nb, void* cb, void* reg) {
   const size_t n = pk->n, fb = pk->fb;
-  RC(d2d(pk->dev, cb, d_lagrange, n * fb));
-  RC(b200_ntt_async(pk->dom0[0], cb, 1, B200_DIF, 0));
-  RC(d2d(pk->dev, reg, cb, n * fb));
-  RC(b200_vec_bit_reverse(pk->dev, pk->curve, reg, pk->logn));
+  RC(to_canonical(pk, d_lagrange, false, cb, reg));
   std::vector<uint8_t> low((size_t)nb * fb);
   RC(b200_d2h(pk->dev, low.data(), reg, (size_t)nb * fb));
   for (int i = 0; i < nb; i++) {       // low coefficients minus b_i (Montgomery form subtracts as is)
@@ -166,6 +183,18 @@ int32_t axpy(b200_plonk_pk_s* pk, void* d_y, const HostFr& a, const void* d_x, s
   return b200_vec_axpy(pk->dev, pk->curve, d_y, ab, d_x, count);
 }
 
+// the polynomials of the batch opening, in the order of BatchedProof.ClaimedValues (:796-807): linearised, l, r, o,
+// s1, s2, then the Qcp_j
+struct Opened { const void* p; size_t count; };
+std::vector<Opened> opened(const b200_plonk_session_s* s) {
+  const b200_plonk_pk_s* pk = s->pk;
+  const size_t n = pk->n;
+  std::vector<Opened> o = {{s->lin, n + 3}, {s->bl[0], n + 2}, {s->bl[1], n + 2}, {s->bl[2], n + 2},
+                           {pk->key[S1].canon, n}, {pk->key[S2].canon, n}};
+  for (uint32_t j = 0; j < pk->n_qcp; j++) o.push_back({pk->key[QCP0 + j].canon, n});
+  return o;
+}
+
 }  // namespace
 
 extern "C" {
@@ -176,11 +205,12 @@ int32_t b200_plonk_pk_free(b200_plonk_pk_t pk) {
   b200_sync(pk->dev);
   for (int i = 0; i < 4; i++) if (pk->dom0[i]) b200_ntt_domain_free(pk->dom0[i]);
   if (pk->dom1) b200_ntt_domain_free(pk->dom1);
-  for (int k = 0; k < 8; k++) { if (pk->br[k]) b200_free(pk->dev, pk->br[k]); if (pk->canon[k]) b200_free(pk->dev, pk->canon[k]); }
   if (pk->d_perm) b200_free(pk->dev, pk->d_perm);
-  for (void* q : pk->qcp_br) if (q) b200_free(pk->dev, q);
-  for (void* q : pk->qcp_canon) if (q) b200_free(pk->dev, q);
-  for (auto& v : pk->key_cos) for (void* q : v) if (q) b200_free(pk->dev, q);
+  for (size_t k = 0; k < pk->key.size(); k++) {
+    std::vector<void*> bufs = {pk->key[k].br, pk->key[k].canon};
+    for (auto& c : pk->key_cos) bufs.push_back(c[k]);
+    for (void* q : bufs) if (q) b200_free(pk->dev, q);
+  }
   if (pk->srs) b200_table_free(pk->srs);
   delete pk;
   return 0;
@@ -192,6 +222,9 @@ int32_t b200_plonk_pk_load(int32_t dev, int32_t curve, const b200_plonk_pk_desc*
   if (!d || !out) return set_error("plonk_pk_load: null argument");
   if (!d->ql || !d->qr || !d->qm || !d->qo || !d->qk || !d->perm || !d->srs_canonical)
     return set_error("plonk_pk_load: null field in the descriptor");
+  if (d->n_qcp > 16 || (d->n_qcp && !d->qcp)) return set_error("plonk_pk_load: invalid BSB22 selector list");
+  for (uint32_t j = 0; j < d->n_qcp; j++)
+    if (!d->qcp[j]) return set_error("plonk_pk_load: null BSB22 selector");
   const NttOps* ops = get_ntt_ops(curve);
   if (!ops) return set_error("plonk_pk_load: unsupported curve");
   if ((int)d->log2n + 2 > ops->two_adicity || d->log2n > 28) return set_error("plonk_pk_load: domain too large");
@@ -228,10 +261,12 @@ int32_t b200_plonk_pk_load(int32_t dev, int32_t curve, const b200_plonk_pk_desc*
     for (size_t i = 0; i < n; i++) { fr->store(wpow.data() + i * fb, acc); acc = fr->mul(acc, pk->w); }
   }
   const HostFr g2 = fr->mul(pk->g, pk->g);
-  const void* lag[8] = {d->ql, d->qr, d->qm, d->qo, d->qk, nullptr, nullptr, nullptr};
-  for (int k = 0; k < 8; k++) {
-    const void* src = lag[k];
-    if (k >= S1) {
+  const void* lag[QCP0] = {d->ql, d->qr, d->qm, d->qo, d->qk, nullptr, nullptr, nullptr};
+  pk->n_qcp = d->n_qcp;
+  pk->key.resize(QCP0 + d->n_qcp);
+  for (size_t k = 0; k < pk->key.size(); k++) {
+    const void* src = k < QCP0 ? lag[k] : d->qcp[k - QCP0];
+    if (k >= S1 && k <= S3) {
       const int j = k - S1;
       for (size_t i = 0; i < n; i++) {
         const uint64_t idx = (uint64_t)d->perm[(size_t)j * n + i];
@@ -242,38 +277,18 @@ int32_t b200_plonk_pk_load(int32_t dev, int32_t curve, const b200_plonk_pk_desc*
       }
       src = sj.data();
     }
-    RC(b200_alloc(dev, n * fb, &pk->br[k]));
-    RC(b200_alloc(dev, n * fb, &pk->canon[k]));
-    RC(b200_h2d(dev, pk->br[k], src, n * fb));
-    RC(b200_ntt_async(pk->dom0[0], pk->br[k], 1, B200_DIF, 0));      // Lagrange/regular -> canonical/bit-reversed
-    RC(d2d(dev, pk->canon[k], pk->br[k], n * fb));
-    RC(b200_vec_bit_reverse(dev, curve, pk->canon[k], d->log2n));
+    RC(b200_alloc(dev, n * fb, &pk->key[k].br));
+    RC(b200_alloc(dev, n * fb, &pk->key[k].canon));
+    RC(to_canonical(pk.get(), src, true, pk->key[k].br, pk->key[k].canon));
   }
-  if (d->n_qcp > 16 || (d->n_qcp && !d->qcp)) return set_error("plonk_pk_load: invalid BSB22 selector list");
-  for (uint32_t j = 0; j < d->n_qcp; j++) {
-    if (!d->qcp[j]) return set_error("plonk_pk_load: null BSB22 selector");
-    void *b = nullptr, *c = nullptr;
-    RC(b200_alloc(dev, n * fb, &b)); pk->qcp_br.push_back(b);
-    RC(b200_alloc(dev, n * fb, &c)); pk->qcp_canon.push_back(c);
-    RC(b200_h2d(dev, b, d->qcp[j], n * fb));
-    RC(b200_ntt_async(pk->dom0[0], b, 1, B200_DIF, 0));
-    RC(d2d(dev, c, b, n * fb));
-    RC(b200_vec_bit_reverse(dev, curve, c, d->log2n));
-  }
-  {
-    const char* e = getenv("GB200_PLONK_COSET_CACHE");
-    if (!e || atoi(e) != 0) {
-      std::vector<void*> src;
-      for (int k = 0; k < 8; k++) src.push_back(pk->br[k]);
-      for (void* q : pk->qcp_br) src.push_back(q);
-      pk->key_cos.assign(4, std::vector<void*>(src.size(), nullptr));
-      for (int i = 0; i < 4; i++)
-        for (size_t k = 0; k < src.size(); k++) {
-          RC(b200_alloc(dev, n * fb, &pk->key_cos[i][k]));
-          RC(d2d(dev, pk->key_cos[i][k], src[k], n * fb));
-          RC(b200_ntt_async(pk->dom0[i], pk->key_cos[i][k], 0, B200_DIT, 1));   // canonical/bit-reversed -> coset i
-        }
-    }
+  const char* e = getenv("GB200_PLONK_COSET_CACHE");
+  if (!e || atoi(e) != 0) {
+    pk->key_cos.assign(4, std::vector<void*>(pk->key.size(), nullptr));
+    for (uint32_t i = 0; i < 4; i++)
+      for (size_t k = 0; k < pk->key.size(); k++) {
+        RC(b200_alloc(dev, n * fb, &pk->key_cos[i][k]));
+        RC(to_coset(pk.get(), i, pk->key[k].br, pk->key_cos[i][k]));
+      }
   }
   RC(b200_table_upload(dev, curve, 1, d->srs_canonical, n + 3, B200_TABLE_PRECOMP, &pk->srs));
   RC(b200_sync(dev));
@@ -298,7 +313,7 @@ int32_t b200_plonk_begin(b200_plonk_pk_t pk, const void* l, const void* r, const
                          b200_plonk_session_t* out, void* out_lro) {
   GUARD_BEGIN
   if (!pk || !l || !r || !o || !bl || !br || !bo || !out || !out_lro) return set_error("plonk_begin: null argument");
-  if (!pk->qcp_br.empty() && (!pi2 || !out_bsb22))
+  if (pk->n_qcp && (!pi2 || !out_bsb22))
     return set_error("plonk_begin: the key has BSB22 commitment gates - one committed polynomial per gate is required");
   const int dev = pk->dev;
   const size_t n = pk->n, fb = pk->fb;
@@ -321,15 +336,12 @@ int32_t b200_plonk_begin(b200_plonk_pk_t pk, const void* l, const void* r, const
   RC(commit_join(pk, d_lro, 3 * s->jb, out_lro));
   // BSB22: committed polynomials -> canonical, and their digests (Bsb22Commitments :300; canonical SRS here, the
   // same group element as the reference's Lagrange-SRS commitment)
-  for (size_t j = 0; j < pk->qcp_br.size(); j++) {
+  for (uint32_t j = 0; j < pk->n_qcp; j++) {
     if (!pi2[j]) return set_error("plonk_begin: null committed polynomial");
     void *b = nullptr, *c = nullptr;
     RC(s->S.alloc(n * fb, &b)); RC(s->S.alloc(n * fb, &c));
     s->pi2_br.push_back(b); s->pi2_canon.push_back(c);
-    RC(b200_h2d(dev, b, pi2[j], n * fb));
-    RC(b200_ntt_async(pk->dom0[0], b, 1, B200_DIF, 0));
-    RC(d2d(dev, c, b, n * fb));
-    RC(b200_vec_bit_reverse(dev, pk->curve, c, pk->logn));
+    RC(to_canonical(pk, pi2[j], true, b, c));
     RC(commit(pk, c, n, (uint8_t*)out_bsb22 + j * s->jb));
   }
   s->stage = 1;
@@ -348,11 +360,7 @@ int32_t b200_plonk_set_qk(b200_plonk_session_t s, const void* qk_lagrange) {
   b200_plonk_pk_s* pk = s->pk;
   const size_t n = pk->n, fb = pk->fb;
   if (!s->qk_br) { RC(s->S.alloc(n * fb, &s->qk_br)); RC(s->S.alloc(n * fb, &s->qk_canon)); }
-  RC(b200_h2d(pk->dev, s->qk_br, qk_lagrange, n * fb));
-  RC(b200_ntt_async(pk->dom0[0], s->qk_br, 1, B200_DIF, 0));       // Lagrange/regular -> canonical/bit-reversed
-  RC(d2d(pk->dev, s->qk_canon, s->qk_br, n * fb));
-  RC(b200_vec_bit_reverse(pk->dev, pk->curve, s->qk_canon, pk->logn));
-  return 0;
+  return to_canonical(pk, qk_lagrange, true, s->qk_br, s->qk_canon);
   GUARD_END
 }
 
@@ -404,18 +412,16 @@ int32_t b200_plonk_quotient(b200_plonk_session_t s, const void* alpha, void* out
   for (int k = 0; k < 12; k++) RC(T.alloc(n * fb, &onc[k]));
   alignas(16) uint8_t gb[8 * HOSTFR_MAX_LIMBS], w4b[8 * HOSTFR_MAX_LIMBS];
   fr->store(gb, pk->g); fr->store(w4b, pk->w4);
-  // argument order of b200_plonk_coset_args: l r o z s1 s2 s3 ql qr qm qo qk
-  const void* srcs[12] = {s->cb[0], s->cb[1], s->cb[2], s->cb[3], pk->br[S1], pk->br[S2], pk->br[S3],
-                          pk->br[QL], pk->br[QR], pk->br[QM], pk->br[QO], s->qk_br ? s->qk_br : pk->br[QK]};
+  // argument order of b200_plonk_coset_args: l r o z, then the key polynomials s1 s2 s3 ql qr qm qo qk
+  const int key_arg[8] = {S1, S2, S3, QL, QR, QM, QO, QK};
   const bool cached = !pk->key_cos.empty();
-  // position of the key polynomials in key_cos[i]: ql qr qm qo qk s1 s2 s3 ; srcs[4..11] = s1 s2 s3 ql qr qm qo qk
-  const int cos_idx[12] = {-1, -1, -1, -1, S1, S2, S3, QL, QR, QM, QO, QK};
   for (uint32_t i = 0; i < 4; i++) {
     const void* on[12];
     for (int k = 0; k < 12; k++) {
-      if (cached && cos_idx[k] >= 0 && !(k == 11 && s->qk_br)) { on[k] = pk->key_cos[i][cos_idx[k]]; continue; }
-      RC(d2d(dev, onc[k], srcs[k], n * fb));
-      RC(b200_ntt_async(pk->dom0[i], onc[k], 0, B200_DIT, 1));     // canonical/bit-reversed -> coset i, regular
+      const int q = k < 4 ? -1 : key_arg[k - 4];
+      if (cached && q >= 0 && !(q == QK && s->qk_br)) { on[k] = pk->key_cos[i][q]; continue; }
+      const void* src = q < 0 ? s->cb[k] : q == QK && s->qk_br ? s->qk_br : pk->key[q].br;
+      RC(to_coset(pk, i, src, onc[k]));
       on[k] = onc[k];
     }
     b200_plonk_coset_args a;
@@ -427,12 +433,10 @@ int32_t b200_plonk_quotient(b200_plonk_session_t s, const void* alpha, void* out
     a.nbl = 2; a.nbr = 2; a.nbo = 2; a.nbz = 3;
     a.coset_index = i; a.rho = 4; a.out = s->h;
     RC(b200_plonk_constraints_coset(pk->dom0[i], gb, w4b, &a));
-    for (size_t j = 0; j < pk->qcp_br.size(); j++) {   // + Qcp_j * PI2_j on this coset (gateConstraint :881-884)
-      const void* qc = onc[0];
-      if (cached) qc = pk->key_cos[i][8 + j];
-      else { RC(d2d(dev, onc[0], pk->qcp_br[j], n * fb)); RC(b200_ntt_async(pk->dom0[i], onc[0], 0, B200_DIT, 1)); }
-      RC(d2d(dev, onc[1], s->pi2_br[j], n * fb));
-      RC(b200_ntt_async(pk->dom0[i], onc[1], 0, B200_DIT, 1));
+    for (uint32_t j = 0; j < pk->n_qcp; j++) {   // + Qcp_j * PI2_j on this coset (gateConstraint :881-884)
+      const void* qc = cached ? pk->key_cos[i][QCP0 + j] : onc[0];
+      if (!cached) RC(to_coset(pk, i, pk->key[QCP0 + j].br, onc[0]));
+      RC(to_coset(pk, i, s->pi2_br[j], onc[1]));
       RC(b200_plonk_bsb22_coset(pk->dom0[i], qc, onc[1], i, 4, s->h));
     }
   }
@@ -486,8 +490,8 @@ int32_t b200_plonk_linearise(b200_plonk_session_t s, const void* zeta_, void* ou
   RC(eval_at(pk, s->bl[0], n + 2, zeta, &lz));
   RC(eval_at(pk, s->bl[1], n + 2, zeta, &rz));
   RC(eval_at(pk, s->bl[2], n + 2, zeta, &oz));
-  RC(eval_at(pk, pk->canon[S1], n, zeta, &s1z));
-  RC(eval_at(pk, pk->canon[S2], n, zeta, &s2z));
+  RC(eval_at(pk, pk->key[S1].canon, n, zeta, &s1z));
+  RC(eval_at(pk, pk->key[S2].canon, n, zeta, &s2z));
   auto M = [&](const HostFr& a, const HostFr& b) { return fr->mul(a, b); };
   auto A = [&](const HostFr& a, const HostFr& b) { return fr->add(a, b); };
   const HostFr rl = M(rz, lz);
@@ -508,16 +512,17 @@ int32_t b200_plonk_linearise(b200_plonk_session_t s, const void* zeta_, void* ou
   void* lin = s->lin;
   RC(dzero(dev, lin, (n + 3) * fb));
   RC(axpy(pk, lin, A(c2, a2l1), s->bl[3], n + 3));
-  RC(axpy(pk, lin, c1, pk->canon[S3], n));
-  RC(axpy(pk, lin, rl, pk->canon[QM], n));
-  RC(axpy(pk, lin, lz, pk->canon[QL], n));
-  RC(axpy(pk, lin, rz, pk->canon[QR], n));
-  RC(axpy(pk, lin, oz, pk->canon[QO], n));
-  RC(axpy(pk, lin, fr->one_(), s->qk_canon ? s->qk_canon : pk->canon[QK], n));
+  RC(axpy(pk, lin, c1, pk->key[S3].canon, n));
+  RC(axpy(pk, lin, rl, pk->key[QM].canon, n));
+  RC(axpy(pk, lin, lz, pk->key[QL].canon, n));
+  RC(axpy(pk, lin, rz, pk->key[QR].canon, n));
+  RC(axpy(pk, lin, oz, pk->key[QO].canon, n));
+  RC(axpy(pk, lin, fr->one_(), s->qk_canon ? s->qk_canon : pk->key[QK].canon, n));
   // + sum_j Qcp_j(zeta) PI2_j(X)   (:1457-1460); Qcp_j(zeta) are claimed values 6.. of the batch opening
-  for (size_t j = 0; j < pk->qcp_canon.size(); j++) {
+  const std::vector<Opened> op = opened(s);
+  for (uint32_t j = 0; j < pk->n_qcp; j++) {
     HostFr qz;
-    RC(eval_at(pk, pk->qcp_canon[j], n, zeta, &qz));
+    RC(eval_at(pk, op[6 + j].p, op[6 + j].count, zeta, &qz));
     fr->store(vals + (7 + j) * fb, qz);
     RC(axpy(pk, lin, qz, s->pi2_canon[j], n));
   }
@@ -540,11 +545,9 @@ int32_t b200_plonk_linearise(b200_plonk_session_t s, const void* zeta_, void* ou
   RC(T.alloc(2 * s->jb, &d_two));
   RC(commit_async(pk, lin, n + 3, d_two));
   // claimed values of the batch opening (BatchedProof.ClaimedValues) - needed by the caller to derive v
-  const void* open_p[6] = {lin, s->bl[0], s->bl[1], s->bl[2], pk->canon[S1], pk->canon[S2]};
-  const size_t open_n[6] = {n + 3, n + 2, n + 2, n + 2, n, n};
   for (int k = 0; k < 6; k++) {
     HostFr e;
-    RC(eval_at(pk, open_p[k], open_n[k], zeta, &e));
+    RC(eval_at(pk, op[k].p, op[k].count, zeta, &e));
     fr->store(vals + (size_t)k * fb, e);
   }
   // Z-shifted opening: (Z(X) - Z(w zeta)) / (X - w zeta)
@@ -564,7 +567,7 @@ int32_t b200_plonk_linearise(b200_plonk_session_t s, const void* zeta_, void* ou
   GUARD_END
 }
 
-// batchOpening :796-837: fold {linearised, l, r, o, s1, s2} with powers of v, divide by X - zeta, commit
+// batchOpening :796-837: fold the opened polynomials with powers of v, divide by X - zeta, commit
 int32_t b200_plonk_batch_open(b200_plonk_session_t s, const void* v_, void* out_point) {
   GUARD_BEGIN
   if (!s || !v_ || !out_point) return set_error("plonk_batch_open: null argument");
@@ -574,19 +577,13 @@ int32_t b200_plonk_batch_open(b200_plonk_session_t s, const void* v_, void* out_
   const int dev = pk->dev, curve = pk->curve;
   const size_t n = pk->n, fb = pk->fb;
   const HostFr v = fr->load(v_);
-  const void* open_p[6] = {s->lin, s->bl[0], s->bl[1], s->bl[2], pk->canon[S1], pk->canon[S2]};
-  const size_t open_n[6] = {n + 3, n + 2, n + 2, n + 2, n, n};
   Scratch T(dev);
   void* fold;
   RC(T.alloc((n + 3) * fb, &fold));
   RC(dzero(dev, fold, (n + 3) * fb));
   HostFr vp = fr->one_();
-  for (int k = 0; k < 6; k++) {
-    RC(axpy(pk, fold, vp, open_p[k], open_n[k]));
-    vp = fr->mul(vp, v);
-  }
-  for (size_t j = 0; j < pk->qcp_canon.size(); j++) {     // polysToOpen[6:] = Qcp (:805-807)
-    RC(axpy(pk, fold, vp, pk->qcp_canon[j], n));
+  for (const Opened& p : opened(s)) {
+    RC(axpy(pk, fold, vp, p.p, p.count));
     vp = fr->mul(vp, v);
   }
   alignas(16) uint8_t rem[8 * HOSTFR_MAX_LIMBS];
@@ -608,7 +605,7 @@ int32_t b200_plonk_prove(b200_plonk_pk_t pk, const void* l, const void* r, const
   const size_t jb = get_msm_ops(pk->curve, 1)->jac_bytes;
   uint8_t* pts = (uint8_t*)out_points;          // L, R, O, Z, H1, H2, H3, linearised, batch opening, Z opening
   b200_plonk_session_t s = nullptr;
-  if (!pk->qcp_br.empty() && (!ch->pi2 || !ch->out_bsb22))
+  if (pk->n_qcp && (!ch->pi2 || !ch->out_bsb22))
     return set_error("plonk_prove: the key has BSB22 commitment gates - challenges.pi2 / out_bsb22 are required");
   using clk = std::chrono::steady_clock;
   auto ms_since = [](clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); };
