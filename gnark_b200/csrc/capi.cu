@@ -159,18 +159,28 @@ int32_t msm_join(DeviceCtx* ctx) {
   return 0;
 }
 
+int msm_window_with_limit(size_t n, int scalar_bits) {
+  int c = msm_window_for(n ? n : 1);
+  while (msm_num_windows(scalar_bits, c) > 64) c++;   // MSM_MAX_WINDOWS of the table precompute
+  return c;
+}
+
 int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* d_scalars, void* d_out,
-                      cudaEvent_t* stage_events, bool pipelined) {
-  if (off + n > t->n) return set_error("msm: range [off, off+n) exceeds the table");
+                      cudaEvent_t* stage_events, bool pipelined, const uint32_t* d_idx) {
+  if (d_idx ? off != 0 : off + n > t->n) return set_error("msm: range [off, off+n) exceeds the table");
+  // a precomputed table's slabs fix its window; an indexed MSM on a plain table sizes its bucket sets by its own n
+  // (a few hundred indices into a 2^22-point table must not pay for 2^15-bucket sets)
+  const int c = (d_idx && !t->precomp) ? msm_window_with_limit(n, t->ops->scalar_bits) : t->c;
+  const int nwin = msm_num_windows(t->ops->scalar_bits, c);
   // the pipeline indexes its n * nwin (scalar, window) entries with 31-bit counts (radix sort, offsets, tasks)
-  if ((size_t)n * (size_t)t->nwin >= ((size_t)1 << 31))
+  if ((size_t)n * (size_t)nwin >= ((size_t)1 << 31))
     return set_error("msm: n * windows exceeds 2^31 entries - split the call into point ranges (or shard the table) and add the results");
   if (stage_events || n == 0) pipelined = false;
   if (!pipelined) { int32_t rc = msm_join(ctx); if (rc) return rc; }
   uint32_t task_len, chunk;
-  msm_tuning(n, t->nwin, t->c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
+  msm_tuning(n, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
   size_t ws_bytes = 0;
-  CK(t->ops->ws_bytes((uint32_t)n, (uint32_t)t->n, t->c, t->precomp, task_len, chunk, &ws_bytes));
+  CK(t->ops->ws_bytes((uint32_t)n, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
   AsyncBuf ws_buf;
   CK(ws_buf.alloc(ws_bytes, ctx->stream));
   void* ws = ws_buf.p;
@@ -186,8 +196,8 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
     pipe.acc_ev = ctx->acc_ev[slot];
     ctx->pipe_seq++;
   }
-  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)t->n, (uint32_t)off, t->c, t->precomp, task_len, chunk,
-                              t->d_points, d_scalars, d_out, ws, stage_events, pipelined ? &pipe : nullptr);
+  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)t->n, (uint32_t)off, c, t->precomp, task_len, chunk,
+                              t->d_points, d_scalars, d_out, ws, stage_events, pipelined ? &pipe : nullptr, d_idx);
   // the workspace is last used by the tail kernels
   cudaError_t e2 = ws_buf.release_on(pipelined ? ctx->tail_stream : ctx->stream);
   if (pipelined && e == cudaSuccess) {
@@ -398,8 +408,7 @@ static int32_t table_new(int dev, int curve, int group, size_t n, int flags, std
   if (!ops) return set_error("table_upload: unsupported curve/group");
   t.reset(new b200_table_s());
   t->dev = dev; t->curve = curve; t->group = group; t->n = n; t->ops = ops;
-  t->c = msm_window_for(n ? n : 1);
-  while (msm_num_windows(ops->scalar_bits, t->c) > 64) t->c++;   // MSM_MAX_WINDOWS of the table precompute
+  t->c = msm_window_with_limit(n, ops->scalar_bits);
   t->nwin = msm_num_windows(ops->scalar_bits, t->c);
   t->precomp = (flags & B200_TABLE_PRECOMP) ? 1 : 0;
   if (env_int("GB200_MSM_PRECOMP", -1) >= 0) t->precomp = env_int("GB200_MSM_PRECOMP", 0) ? 1 : 0;

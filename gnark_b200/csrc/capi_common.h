@@ -77,8 +77,13 @@ namespace gb200 {
 // cudaMalloc / cudaFree (b200_alloc / b200_free: synchronous, unmap on free) were a visible part of its wall time
 int32_t scratch_alloc(int dev, size_t bytes, void** out);
 int32_t scratch_free(int dev, void* p);
+// d_idx (optional, device): n table indices already checked against t->n; scalar i then multiplies base d_idx[i]
+// (off must be 0).  On a plain table an indexed MSM takes its window from n, not from the table's size.
 int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* d_scalars, void* d_out,
-                      cudaEvent_t* stage_events = nullptr, bool pipelined = false);
+                      cudaEvent_t* stage_events = nullptr, bool pipelined = false, const uint32_t* d_idx = nullptr);
+// window of an MSM of n scalars on a table of `scalar_bits`-bit scalars: msm_window_for(n), raised until the scalar has
+// at most 64 windows (MSM_MAX_WINDOWS of the table precompute)
+int msm_window_with_limit(size_t n, int scalar_bits);
 int32_t msm_join(DeviceCtx* ctx);  // make ctx->stream wait for the pipelined tails
 
 // Buffers of one synchronous entry point, all on ctx->stream.  Host pointers are borrowed for the call only: host

@@ -138,3 +138,55 @@ int32_t b200_msm_gather(b200_table_t t, size_t off, const uint32_t* idx, size_t 
 }
 
 }  // extern "C"
+
+// first_bad = the lowest position j < n with idx[j] >= count (stays 0xffffffff when every index is valid)
+static __global__ void __launch_bounds__(256) k_msm_check_indices(const uint32_t* __restrict__ idx, uint32_t n,
+                                                                  uint32_t count, uint32_t* __restrict__ first_bad) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n && !msm_index_ok(idx, j, count)) atomicMin(first_bad, j);
+}
+
+extern "C" {
+
+// sum_j scalars[j] * bases[idx[j]], j < n: the bases are picked from the table through the index list (any order, repeats
+// allowed) - a sparse vector committed against a whole table (the BSB22 hint's kzg.Commit over pk.KzgLagrange,
+// backend/plonk/bn254/prove.go:280-315) at a cost that follows n, not the table size.  Every index is checked before any
+// kernel reads a point through it: host indices here, device indices by k_msm_check_indices, whose verdict is downloaded
+// (one synchronisation) before the MSM is enqueued.
+int32_t b200_msm_indexed(b200_table_t t, const uint32_t* idx, size_t n, int32_t idx_on_device, const void* scalars,
+                         int32_t scalars_on_device, void* out_jac_host) {
+  GUARD_BEGIN
+  if (!t) return set_error("msm_indexed: null table");
+  if (!out_jac_host || (n && (!idx || !scalars))) return set_error("msm_indexed: null argument");
+  if (n >= ((size_t)1 << 31)) return set_error("msm_indexed: n * windows exceeds 2^31 entries - split the call and add the results");
+  GB_DEVICE(ctx, t->dev);
+  if (!idx_on_device)
+    for (size_t j = 0; j < n; j++)
+      if (idx[j] >= t->n)
+        return set_error("msm_indexed: index " + std::to_string(idx[j]) + " out of range at position " + std::to_string(j) +
+                         " (table of " + std::to_string(t->n) + " points)");
+  Staging st(ctx);
+  void* d_out;
+  const void *sc, *ix;
+  CK(st.out(out_jac_host, t->ops->jac_bytes, false, &d_out));
+  CK(st.in(idx, n * sizeof(uint32_t), idx_on_device, &ix));
+  CK(st.in(scalars, n * t->ops->fr_bytes, scalars_on_device, &sc));
+  if (idx_on_device && n) {
+    void* d_bad;
+    uint32_t bad = 0;
+    CK(st.scratch(sizeof(uint32_t), &d_bad));
+    CK(cudaMemsetAsync(d_bad, 0xff, sizeof(uint32_t), ctx->stream));
+    k_msm_check_indices<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(static_cast<const uint32_t*>(ix), (uint32_t)n,
+                                                                             (uint32_t)t->n, static_cast<uint32_t*>(d_bad));
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (bad != 0xffffffffu)
+      return st.finish("msm_indexed", set_error("msm_indexed: device index out of range at position " + std::to_string(bad) +
+                                                " (table of " + std::to_string(t->n) + " points)"));
+  }
+  return st.finish("msm_indexed", msm_on_stream(ctx, t, 0, n, sc, d_out, nullptr, false, static_cast<const uint32_t*>(ix)));
+  GUARD_END
+}
+
+}  // extern "C"

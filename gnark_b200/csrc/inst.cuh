@@ -30,12 +30,12 @@ struct MsmInst {
   }
   static cudaError_t run(cudaStream_t st, uint32_t n, uint32_t stride, uint32_t off, int c, int precomp,
                          uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars,
-                         void* d_out_jac, void* ws, cudaEvent_t* ev, const MsmPipe* pipe) {
+                         void* d_out_jac, void* ws, cudaEvent_t* ev, const MsmPipe* pipe, const uint32_t* d_idx) {
     MsmPlan pl = plan(n, stride, off, c, precomp, task_len, chunk);
     MsmLayout<F> L;
     GB_CUDA_TRY(msm_layout<F>(pl, L));
     return msm_enqueue<Fr, F>(st, pl, reinterpret_cast<const Affine<F>*>(d_table),
-                              reinterpret_cast<const Fr*>(d_scalars), reinterpret_cast<Jacobian<F>*>(d_out_jac), ws, L, ev, pipe);
+                              reinterpret_cast<const Fr*>(d_scalars), reinterpret_cast<Jacobian<F>*>(d_out_jac), ws, L, ev, pipe, d_idx);
   }
   // d_table holds the n bases in slab 0 already; slabs 1.. are filled in place
   static cudaError_t precompute(cudaStream_t st, uint32_t n, int nwin, int c, void* d_table) {

@@ -44,11 +44,12 @@ struct MsmOps {
   size_t jac_bytes;     // sizeof(G?Jac)
   // workspace bytes for an MSM of n scalars with the given parameters
   cudaError_t (*ws_bytes)(uint32_t n, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk, size_t* out);
-  // enqueue a full MSM (all pointers on device)
+  // enqueue a full MSM (all pointers on device); d_idx null: bases off + i, else bases d_idx[i] (indices checked
+  // against the table's point count by the caller)
   cudaError_t (*run)(cudaStream_t st, uint32_t n, uint32_t stride, uint32_t off, int c, int precomp,
                      uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars, void* d_out_jac,
                      void* ws, cudaEvent_t* stage_events /* nullable, 8 entries */,
-                     const MsmPipe* pipe /* nullable: everything on st */);
+                     const MsmPipe* pipe /* nullable: everything on st */, const uint32_t* d_idx);
   // fill slabs 1..nwin-1 of a [nwin][n] table whose slab 0 holds the bases
   cudaError_t (*precompute)(cudaStream_t st, uint32_t n, int nwin, int c, void* d_table);
   // resident 128-thread blocks of the accumulate kernel per SM (occupancy API): the task length is chosen so that the

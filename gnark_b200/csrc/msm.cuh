@@ -56,12 +56,20 @@ HD MsmPlan msm_make_plan(uint32_t n, uint32_t table_stride, uint32_t table_off, 
   return p;
 }
 
+// ---- 0. index check (indexed MSMs) -------------------------------------------
+// an index list may address the table only through checked entries: position i is valid when it names one of the
+// table's `count` points (not slab entries: the slab offset is added by the decompose)
+HD bool msm_index_ok(const uint32_t* idx, uint32_t i, uint32_t count) { return idx[i] < count; }
+
 // ---- 1. decompose ----------------------------------------------------------
-// keys/vals are laid out [w][i] (coalesced per window).  val = table index | sign<<31.
+// keys/vals are laid out [w][i] (coalesced per window).  val = table index | sign<<31.  The base of scalar i is
+// table_off + i, or idx[i] when an index list is given (checked by msm_index_ok before the MSM is enqueued).
 template <class Fr>
-HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint32_t* keys, uint32_t* vals) {
+HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint32_t* keys, uint32_t* vals,
+                          const uint32_t* idx = nullptr) {
   constexpr int N = Fr::N;
   const Fr s = scalars[i].from_mont();
+  const uint32_t base = idx ? idx[i] : pl.table_off + i;
   uint32_t carry = 0;
   const uint32_t half = pl.set_size;  // 2^(c-1)
   const uint32_t mask = (pl.c == 32) ? 0xffffffffu : ((1u << pl.c) - 1u);
@@ -88,8 +96,8 @@ HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint
     } else {
       const uint32_t set = pl.precomp ? 0u : (uint32_t)w;
       keys[slot] = set * pl.set_size + (d - 1);
-      const uint32_t idx = (pl.precomp ? (uint32_t)w * pl.table_stride : 0u) + pl.table_off + i;
-      vals[slot] = idx | (neg << 31);
+      const uint32_t ti = (pl.precomp ? (uint32_t)w * pl.table_stride : 0u) + base;
+      vals[slot] = ti | (neg << 31);
     }
   }
 }

@@ -19,11 +19,13 @@ namespace gb200 {
 // ---------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------
+// idx: null (bases table_off + i) or the checked index list of an indexed MSM (bases idx[i])
 template <class Fr>
 __global__ void __launch_bounds__(256) k_msm_decompose(MsmPlan pl, const Fr* __restrict__ scalars,
-                                                       uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+                                                       uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                       const uint32_t* __restrict__ idx) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < pl.n) msm_decompose_one<Fr>(pl, i, scalars, keys, vals);
+  if (i < pl.n) msm_decompose_one<Fr>(pl, i, scalars, keys, vals, idx);
 }
 
 // off[b] = first sorted position with key >= b, for b in [0, nb]
@@ -354,11 +356,12 @@ inline int msm_set_sum_threads(size_t budget = 160 * 1024) {
 }
 
 // Enqueue a full MSM on `stream`.  d_scalars: n Fr elements (Montgomery) on device.
-// d_out: one Jacobian<F> on device.  ws must hold msm_layout().total bytes.
+// d_out: one Jacobian<F> on device.  ws must hold msm_layout().total bytes.  d_idx (optional): n checked table indices,
+// scalar i then multiplies base d_idx[i] instead of base table_off + i.
 template <class Fr, class F>
 cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>* d_table, const Fr* d_scalars,
                         Jacobian<F>* d_out, void* ws, const MsmLayout<F>& L, cudaEvent_t* ev = nullptr,
-                        const MsmPipe* pipe = nullptr) {
+                        const MsmPipe* pipe = nullptr, const uint32_t* d_idx = nullptr) {
   // pipe (optional, internal.h): the accumulate kernel and the latency-bound reduction kernels that follow it are
   // enqueued on their own streams (forked with events), so that in a pipeline of MSMs the next MSM's DRAM-bound
   // front overlaps this one's multiplier-bound accumulate, and the tail overlaps both instead of idling most of the SMs.
@@ -387,7 +390,7 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
     return cudaGetLastError();
   }
   GB_EV(0);
-  k_msm_decompose<Fr><<<(pl.n + 255) / 256, 256, 0, stream>>>(pl, d_scalars, keys0, vals0);
+  k_msm_decompose<Fr><<<(pl.n + 255) / 256, 256, 0, stream>>>(pl, d_scalars, keys0, vals0, d_idx);
   GB_EV(1);
   int end_bit = 1;
   while ((1ull << end_bit) <= nb) end_bit++;

@@ -39,7 +39,7 @@ EXPORTS = [
     "b200_comm_unique_id", "b200_comm_init", "b200_comm_init_all", "b200_comm_destroy", "b200_comm_info",
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
-    "b200_points_ntt",
+    "b200_points_ntt", "b200_msm_indexed",
 ]
 COMM_ID_BYTES = 128
 
@@ -156,6 +156,8 @@ def load(path: str = None):
         lib.b200_pedersen_key_free.argtypes = [vp]
         lib.b200_pedersen_commit.argtypes = [vp, vp, sz, i32, vp, vp]
         lib.b200_pedersen_fold.argtypes = [i32, vp, sz, vp, vp]
+    if "b200_msm_indexed" not in missing:
+        lib.b200_msm_indexed.argtypes = [vp, vp, sz, i32, vp, i32, vp]
     if "b200_table_upload_encoded" not in missing:
         lib.b200_table_upload_encoded.argtypes = [i32, i32, i32, vp, sz, i32, i32, ctypes.POINTER(vp)]
     if "b200_plonk_set_qk" not in missing:
@@ -387,6 +389,24 @@ class Table:
         out = np.zeros(3 * self.coord_limbs, dtype=np.uint64)
         check(load().b200_msm_gather(self.handle, off, ptr(idx), n_idx, 1 if idx_dev else 0, ptr(scalars), n_sc,
                                      1 if sc_dev else 0, ptr(out)))
+        return out
+
+    def msm_indexed(self, idx, scalars) -> np.ndarray:
+        """sum_j scalars[j] * bases[idx[j]] -> Jacobian (gnark layout): the bases picked by index (any order, repeats
+        allowed, each below the table's point count), e.g. kzg.Commit of a sparse Lagrange-form vector.  idx: uint32 host
+        array or int32/uint32 device tensor; scalars: (len(idx), fr_limbs) host array or device tensor"""
+        idx_dev, sc_dev = hasattr(idx, "data_ptr"), hasattr(scalars, "data_ptr")
+        n = idx.numel() if idx_dev else np.asarray(idx).size
+        if not idx_dev:
+            idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        if not sc_dev:
+            scalars = np.ascontiguousarray(scalars, dtype=np.uint64)
+        n_sc = (scalars.numel() if sc_dev else scalars.size) // self.fr_limbs
+        if n_sc != n:
+            raise ValueError(f"msm_indexed: {n} indices and {n_sc} scalars")
+        out = np.zeros(3 * self.coord_limbs, dtype=np.uint64)
+        check(load().b200_msm_indexed(self.handle, ptr(idx), n, 1 if idx_dev else 0, ptr(scalars), 1 if sc_dev else 0,
+                                      ptr(out)))
         return out
 
     def msm_async(self, d_scalars, d_out, off: int = 0, n: int = None):

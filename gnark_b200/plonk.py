@@ -235,6 +235,35 @@ class ProvingKey:
             self.srs.free()
 
 
+def bsb22_commitment(lagrange_table, nb_public: int, committed, values, blind2):
+    """The commitment of the BSB22 solver hint (bsb22Hint, backend/plonk/bn254/prove.go:280-315) and its committed
+    polynomial.  The hint's vector has n = lagrange_table.n entries (Lagrange form, regular layout) and is zero except:
+      nb_public + committed[i]  <- values[i]     (the committed wires, ci.Committed)
+      nb_public + p             <- v             for each (p, v) of blind2: the two blinding values, at the commitment
+                                                 constraint ci.CommitmentIndex and at the last constraint nbConstraints - 1
+    written in that order (a later write replaces an earlier one, as in the hint).  The digest kzg.Commit(vector,
+    pk.KzgLagrange) is one indexed MSM over those few entries (Table.msm_indexed), not an MSM over n scalars.
+    values: (len(committed), fr_limbs) Montgomery; blind2: two (constraint index, Montgomery value).
+    Returns (digest as a Jacobian point in gnark layout, the dense (n, fr_limbs) vector that Prove(..., pi2=) takes)."""
+    L = lagrange_table.fr_limbs
+    values = np.ascontiguousarray(values, dtype=np.uint64).reshape(-1, L)
+    if len(committed) != values.shape[0]:
+        raise ValueError(f"{len(committed)} committed wires and {values.shape[0]} values")
+    if len(blind2) != 2:
+        raise ValueError("the hint blinds exactly two entries")
+    entries = {}
+    for p, v in list(zip(committed, values)) + [(p, np.asarray(v, dtype=np.uint64).reshape(L)) for p, v in blind2]:
+        pos = nb_public + int(p)
+        if not 0 <= pos < lagrange_table.n:
+            raise ValueError(f"position {pos} outside the {lagrange_table.n}-point Lagrange basis")
+        entries[pos] = v
+    idx = np.fromiter(entries.keys(), dtype=np.uint32, count=len(entries))
+    sc = np.ascontiguousarray(np.stack(list(entries.values())), dtype=np.uint64)
+    dense = np.zeros((lagrange_table.n, L), dtype=np.uint64)
+    dense[idx] = sc
+    return lagrange_table.msm_indexed(idx, sc), dense
+
+
 def Prove(pk: ProvingKey, l, r, o, ch: Challenges, pi2=()) -> Proof:
     """l, r, o: (n, limbs) uint64 Lagrange/regular solution vectors (SparseR1CSSolution{L,R,O},
     constraint/bn254/system.go:208-210) on the host; pi2: one (n, limbs) Lagrange/regular vector per BSB22

@@ -315,3 +315,43 @@ func PointsNTT(dev int, curve int32, log2n uint32, points unsafe.Pointer, invers
 	}
 	return Call(func() int32 { return int32(C.b200_points_ntt(d, 1, points, 0, inv)) })
 }
+
+// Table is a device-resident MSM base table (b200_table_t).
+type Table struct {
+	h C.b200_table_t
+	N int
+}
+
+// UploadTable is b200_table_upload: n affine points of `group` (1 or 2) from host memory (borrowed for the call).
+// flags: 0 for a plain table, TablePrecomp for one with the precomputed window slabs.
+func UploadTable(dev int, curve, group int32, points unsafe.Pointer, n int, flags int32) (*Table, error) {
+	t := &Table{N: n}
+	err := Call(func() int32 {
+		return int32(C.b200_table_upload(C.int32_t(dev), C.int32_t(curve), C.int32_t(group), points, C.size_t(n), C.int32_t(flags), &t.h))
+	})
+	if err != nil {
+		return nil, err
+	}
+	return t, nil
+}
+
+// MSMIndexed is b200_msm_indexed: sum_j scalars[j] * bases[idx[j]] into out (one G?Jac). idx and scalars (len(idx)
+// fr.Elements) are host memory borrowed for the call; every index must be below the table's point count.
+func (t *Table) MSMIndexed(idx []uint32, scalars, out unsafe.Pointer) error {
+	var pinner runtime.Pinner
+	defer pinner.Unpin()
+	var ip *C.uint32_t
+	if len(idx) > 0 {
+		pinner.Pin(unsafe.SliceData(idx))
+		ip = (*C.uint32_t)(unsafe.SliceData(idx))
+	}
+	return Call(func() int32 { return int32(C.b200_msm_indexed(t.h, ip, C.size_t(len(idx)), 0, scalars, 0, out)) })
+}
+
+// Free is b200_table_free; safe on a nil table and more than once.
+func (t *Table) Free() {
+	if t != nil && t.h != nil {
+		C.b200_table_free(t.h)
+		t.h = nil
+	}
+}

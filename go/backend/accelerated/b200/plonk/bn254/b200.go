@@ -53,7 +53,7 @@ func (pk *ProvingKey) setupDevicePointers(spr *cs.SparseR1CS, domain0 *fft.Domai
 		if pk.deviceInfo.spr == spr && pk.deviceInfo.device == cfg.DeviceID {
 			return nil
 		}
-		pk.deviceInfo.key.Free()
+		pk.deviceInfo.free()
 		pk.deviceInfo = nil
 	}
 	n := int(domain0.Cardinality)
@@ -75,7 +75,24 @@ func (pk *ProvingKey) setupDevicePointers(spr *cs.SparseR1CS, domain0 *fft.Domai
 	if err != nil {
 		return err
 	}
-	pk.deviceInfo = &deviceInfo{spr: spr, device: cfg.DeviceID, key: key, trace: trace}
+	// the BSB22 hint commits against the Lagrange SRS (kzg.Commit(values, pk.KzgLagrange), prove.go:300): a plain table
+	// of exactly n points, as plonk.Setup requires; systems without commitments upload nothing more
+	var lagrange *cabi.Table
+	if len(trace.Qcp) > 0 {
+		if len(pk.KzgLagrange.G1) != n {
+			key.Free()
+			return fmt.Errorf("kzg lagrange srs: %d points, need %d", len(pk.KzgLagrange.G1), n)
+		}
+		var pinner runtime.Pinner
+		pinner.Pin(unsafe.SliceData(pk.KzgLagrange.G1))
+		lagrange, err = cabi.UploadTable(cfg.DeviceID, curveID, 1, ptrOf(pk.KzgLagrange.G1), n, 0)
+		pinner.Unpin()
+		if err != nil {
+			key.Free()
+			return err
+		}
+	}
+	pk.deviceInfo = &deviceInfo{spr: spr, device: cfg.DeviceID, key: key, trace: trace, lagrange: lagrange}
 	return nil
 }
 
@@ -195,8 +212,9 @@ func Prove(spr *cs.SparseR1CS, pk *ProvingKey, fullWitness witness.Witness, cfg 
 	fs := fiatshamir.NewTranscript(opt.ChallengeHash, "gamma", "beta", "alpha", "zeta")
 
 	// BSB22 commitments (initBSB22Commitments + bsb22Hint, prove.go:268-318): the hint runs while solving, before
-	// L, R, O exist, so its commitment is the Lagrange-SRS MSM of the reference; the committed polynomials are kept and
-	// handed to the device prover, which adds their gate term, their part of the linearised polynomial and the openings
+	// L, R, O exist, so its commitment is the Lagrange-SRS MSM of the reference - here one indexed MSM on the device over
+	// the hint's few non-zero entries (b200_msm_indexed); the committed polynomials are kept and handed to the device
+	// prover, which adds their gate term, their part of the linearised polynomial and the openings
 	commitmentInfo := spr.CommitmentInfo.(constraint.PlonkCommitments)
 	commitmentVal := make([]fr.Element, len(commitmentInfo))
 	committed := make([][]fr.Element, len(commitmentInfo))
@@ -220,10 +238,31 @@ func Prove(spr *cs.SparseR1CS, pk *ProvingKey, fullWitness witness.Witness, cfg 
 				return err
 			}
 			committed[commDepth] = values
-			var err error
-			if proof.Bsb22Commitments[commDepth], err = kzg.Commit(values, pk.KzgLagrange); err != nil {
+			// kzg.Commit(values, pk.KzgLagrange) over the len(ins) + 2 entries the hint wrote (a position written twice
+			// is taken once, with its last value, as in the dense vector)
+			positions := append(append(make([]int, 0, len(ins)+2), ci.Committed[:len(ins)]...), ci.CommitmentIndex, spr.GetNbConstraints()-1)
+			idx := make([]uint32, 0, len(positions))
+			seen := make(map[int]bool, len(positions))
+			for _, p := range positions {
+				if !seen[p] {
+					seen[p] = true
+					idx = append(idx, uint32(offset+p))
+				}
+			}
+			scalars := make([]fr.Element, len(idx))
+			for j, p := range idx {
+				scalars[j] = values[p]
+			}
+			var digest curve.G1Jac
+			var pinner runtime.Pinner
+			pinner.Pin(unsafe.SliceData(scalars))
+			pinner.Pin(&digest)
+			err := info.lagrange.MSMIndexed(idx, ptrOf(scalars), unsafe.Pointer(&digest))
+			pinner.Unpin()
+			if err != nil {
 				return err
 			}
+			proof.Bsb22Commitments[commDepth].FromJacobian(&digest)
 			opt.HashToFieldFn.Write(proof.Bsb22Commitments[commDepth].Marshal())
 			hashBts := opt.HashToFieldFn.Sum(nil)
 			opt.HashToFieldFn.Reset()
@@ -302,7 +341,7 @@ func Prove(spr *cs.SparseR1CS, pk *ProvingKey, fullWitness witness.Witness, cfg 
 	for i := range lro {
 		proof.LRO[i].FromJacobian(&lro[i])
 	}
-	for i := range bsbJac { // the device's [PI2_i] must be the hint's commitment
+	for i := range bsbJac { // two independent device paths must agree: the hint's indexed Lagrange MSM and [PI2_i] of the canonical form
 		var d kzg.Digest
 		d.FromJacobian(&bsbJac[i])
 		if !d.Equal(&proof.Bsb22Commitments[i]) {

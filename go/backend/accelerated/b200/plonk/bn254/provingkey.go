@@ -14,12 +14,19 @@ import (
 )
 
 // deviceInfo is the device-resident form of the key: the trace (Ql, Qr, Qm, Qo, Qk, Qcp, the permutation) of ONE
-// constraint system and the canonical KZG SRS, behind b200_plonk_pk_load.
+// constraint system and the canonical KZG SRS, behind b200_plonk_pk_load; and, when the system has BSB22 commitments,
+// pk.KzgLagrange.G1 as a plain table for the hint's commitment (b200_msm_indexed).
 type deviceInfo struct {
-	spr    *cs.SparseR1CS // the system the trace was built from
-	device int
-	key    *cabi.PlonkKey
-	trace  *plonk_bn254.Trace
+	spr      *cs.SparseR1CS // the system the trace was built from
+	device   int
+	key      *cabi.PlonkKey
+	trace    *plonk_bn254.Trace
+	lagrange *cabi.Table // nil without BSB22 commitments
+}
+
+func (d *deviceInfo) free() {
+	d.key.Free()
+	d.lagrange.Free()
 }
 
 // ProvingKey embeds the native key so that WriteTo / ReadFrom are inherited and keys are wire compatible with the CPU
@@ -36,7 +43,7 @@ func (pk *ProvingKey) FreeGPUResources() {
 	pk.setupMu.Lock()
 	defer pk.setupMu.Unlock()
 	if pk.deviceInfo != nil {
-		pk.deviceInfo.key.Free()
+		pk.deviceInfo.free()
 		pk.deviceInfo = nil
 	}
 }

@@ -178,6 +178,16 @@ int32_t b200_msm_allreduce(b200_table_t bases, size_t off, size_t n, const void*
  * icicle.go:1018-1070).  idx / scalars: host or device memory. */
 int32_t b200_msm_gather(b200_table_t bases, size_t off, const uint32_t* idx, size_t n_idx, int32_t idx_on_device,
                         const void* scalars_mont, size_t n_scalars, int32_t scalars_on_device, void* out_jac_host);
+/* sum_{j<n} scalars[j] * bases[idx[j]]: bases picked from the table by index (any order, repeats allowed, each < the
+ * table's point count); idx / scalars host or device; out: one G?Jac on the host.  The sparse twin of b200_msm
+ * (e.g. kzg.Commit of a mostly-zero Lagrange-form vector, the BSB22 hint) - cost follows n, not the table size.
+ * b200_msm_gather indexes the other side: there the scalars are picked (scalars[idx[j]]) and the bases are a
+ * contiguous range.  On a plain table the window comes from n; a precomputed table keeps the window its slabs were
+ * built for.  Every index is checked before a point is read: host indices on the host, device indices by a check
+ * kernel whose verdict is downloaded (one synchronisation) before the MSM runs.  An index out of range fails the call,
+ * names its position and leaves out_jac_host untouched.  n = 0 gives the point at infinity. */
+int32_t b200_msm_indexed(b200_table_t bases, const uint32_t* idx, size_t n, int32_t idx_on_device,
+                         const void* scalars_mont, int32_t scalars_on_device, void* out_jac_host);
 
 /* Pedersen / BSB22 commitment keys (gnark-crypto pedersen.ProvingKey{Basis, BasisExpSigma}, one per commitment:
  * ProvingKey.CommitmentKeys, backend/groth16/bn254/setup.go:46).  b200_pedersen_commit runs
