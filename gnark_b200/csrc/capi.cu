@@ -95,9 +95,10 @@ int msm_window_for(size_t n) {
   if (c > 16) c = 16;
   return c;
 }
-void msm_tuning(size_t n, int nwin, int c, int precomp, int acc_blocks_per_sm, uint32_t* task_len, uint32_t* chunk) {
-  const size_t m = n * (size_t)nwin;
-  const size_t buckets = (precomp ? (size_t)1 : (size_t)nwin) << (c - 1);
+void msm_tuning(size_t n, size_t batch, int nwin, int c, int precomp, int acc_blocks_per_sm, uint32_t* task_len,
+                uint32_t* chunk) {
+  const size_t m = n * batch * (size_t)nwin;
+  const size_t buckets = batch * (precomp ? (size_t)1 : (size_t)nwin) << (c - 1);
   // Task length.  One thread adds a task's entries; a bucket of k entries is cut into ceil(k / task_len) tasks.  Short
   // tasks fill the machine evenly (the accumulate grid is many waves deep, the short last task of every bucket idles its
   // lane for less) at the price of more partial sums for the combine kernel.  Within [24, 40] ([48, 64] for grids of a
@@ -178,9 +179,9 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
   if (stage_events || n == 0) pipelined = false;
   if (!pipelined) { int32_t rc = msm_join(ctx); if (rc) return rc; }
   uint32_t task_len, chunk;
-  msm_tuning(n, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
+  msm_tuning(n, 1, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
   size_t ws_bytes = 0;
-  CK(t->ops->ws_bytes((uint32_t)n, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
+  CK(t->ops->ws_bytes((uint32_t)n, 1, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
   AsyncBuf ws_buf;
   CK(ws_buf.alloc(ws_bytes, ctx->stream));
   void* ws = ws_buf.p;
@@ -196,7 +197,7 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
     pipe.acc_ev = ctx->acc_ev[slot];
     ctx->pipe_seq++;
   }
-  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)t->n, (uint32_t)off, c, t->precomp, task_len, chunk,
+  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, 1, (uint32_t)t->n, (uint32_t)off, c, t->precomp, task_len, chunk,
                               t->d_points, d_scalars, d_out, ws, stage_events, pipelined ? &pipe : nullptr, d_idx);
   // the workspace is last used by the tail kernels
   cudaError_t e2 = ws_buf.release_on(pipelined ? ctx->tail_stream : ctx->stream);
@@ -642,6 +643,47 @@ int32_t b200_msm(b200_table_t t, size_t off, size_t n, const void* scalars, int3
   CK(st.out(out_host, t->ops->jac_bytes, false, &d_out));
   CK(st.in(scalars, n * t->ops->fr_bytes, on_dev, &sc));
   return st.finish("msm", msm_on_stream(ctx, t, off, n, sc, d_out));
+  GUARD_END
+}
+
+// out[b] = sum_i scalars[b * n + i] * bases[off + i], b < batch: the batch runs as ONE MSM whose bucket sets are the
+// items' sets side by side (msm_make_batch_plan) - one decompose, sort and accumulate, one reduction tail whose finish
+// runs the items' Horner sums in parallel - instead of `batch` calls that each pay the latency-bound tail and a sync.
+int32_t b200_msm_batch(b200_table_t t, size_t off, size_t n, size_t batch, const void* scalars, int32_t on_dev,
+                       void* out_host) {
+  GUARD_BEGIN
+  if (!t) return set_error("msm_batch: null table");
+  if (!out_host || (batch && n && !scalars)) return set_error("msm_batch: null argument");
+  if (off > t->n || n > t->n - off) return set_error("msm_batch: range [off, off+n) exceeds the table");
+  if (batch == 0) return 0;
+  // a precomputed table's slabs fix its window; on a plain table the window follows n, as for an indexed MSM (a batch of
+  // short vectors against a long SRS must not pay for the table's 2^15-bucket sets)
+  const int bits = t->ops->scalar_bits;
+  const int c = t->precomp ? t->c : msm_window_with_limit(n, bits);
+  const int nwin = msm_num_windows(bits, c);
+  const unsigned __int128 entries = (unsigned __int128)batch * n * (unsigned)nwin;
+  if (entries >= ((unsigned __int128)1 << 31))
+    return set_error("msm_batch: batch * n * windows exceeds 2^31 entries - split the batch into smaller ones");
+  // bucket keys are 32-bit with the batch's bucket count as the "no entry" key, and the bucket scan counts them in an int
+  const unsigned __int128 buckets = ((unsigned __int128)batch * (t->precomp ? 1u : (unsigned)nwin)) << (c - 1);
+  if (buckets >= ((unsigned __int128)1 << 31) - 1)
+    return set_error("msm_batch: batch * bucket sets * 2^(c-1) exceeds 2^31 - 2 bucket keys - split the batch into "
+                     "smaller ones");
+  GB_DEVICE(ctx, t->dev);
+  int32_t rc = msm_join(ctx); if (rc) return rc;
+  uint32_t task_len, chunk;
+  msm_tuning(n, batch, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
+  size_t ws_bytes = 0;   // n = 0 writes `batch` points at infinity and needs no workspace
+  if (n) CK(t->ops->ws_bytes((uint32_t)n, (uint32_t)batch, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
+  Staging st(ctx);
+  void *d_out, *ws;
+  const void* sc;
+  CK(st.out(out_host, batch * t->ops->jac_bytes, false, &d_out));
+  CK(st.in(scalars, batch * n * t->ops->fr_bytes, on_dev, &sc));
+  CK(st.scratch(ws_bytes, &ws));
+  return st.finish("msm_batch", t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)batch, (uint32_t)t->n, (uint32_t)off, c,
+                                            t->precomp, task_len, chunk, t->d_points, sc, d_out, ws, nullptr, nullptr,
+                                            nullptr));
   GUARD_END
 }
 

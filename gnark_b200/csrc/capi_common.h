@@ -50,7 +50,8 @@ int32_t set_error(const std::string& msg);
 int32_t cuda_fail(const char* what, cudaError_t e);
 int32_t device_ctx(int dev, DeviceCtx** out);
 int msm_window_for(size_t n);
-void msm_tuning(size_t n, int nwin, int c, int precomp, int acc_blocks_per_sm, uint32_t* task_len, uint32_t* chunk);
+// task length and reduction chunk of `batch` MSMs of n scalars each (1: a single MSM), sized by their total entries and buckets
+void msm_tuning(size_t n, size_t batch, int nwin, int c, int precomp, int acc_blocks_per_sm, uint32_t* task_len, uint32_t* chunk);
 
 }  // namespace gb200
 

@@ -17,21 +17,22 @@ namespace gb200 {
 // ---------------------------------------------------------------------------
 template <class Fr, class F>
 struct MsmInst {
-  static MsmPlan plan(uint32_t n, uint32_t stride, uint32_t off, int c, int precomp, uint32_t task_len,
+  static MsmPlan plan(uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp, uint32_t task_len,
                       uint32_t chunk) {
-    return msm_make_plan(n, stride, off, Fr::Params::BITS, c, precomp, task_len, chunk);
+    return msm_make_batch_plan(batch, n, stride, off, Fr::Params::BITS, c, precomp, task_len, chunk);   // batch 1: msm_make_plan's
   }
-  static cudaError_t ws_bytes(uint32_t n, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk, size_t* out) {
+  static cudaError_t ws_bytes(uint32_t n, uint32_t batch, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk,
+                              size_t* out) {
     MsmLayout<F> L;
-    MsmPlan pl = plan(n, stride, 0, c, precomp, task_len, chunk);
+    MsmPlan pl = plan(n, batch, stride, 0, c, precomp, task_len, chunk);
     GB_CUDA_TRY(msm_layout<F>(pl, L));
     *out = L.total;
     return cudaSuccess;
   }
-  static cudaError_t run(cudaStream_t st, uint32_t n, uint32_t stride, uint32_t off, int c, int precomp,
+  static cudaError_t run(cudaStream_t st, uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp,
                          uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars,
                          void* d_out_jac, void* ws, cudaEvent_t* ev, const MsmPipe* pipe, const uint32_t* d_idx) {
-    MsmPlan pl = plan(n, stride, off, c, precomp, task_len, chunk);
+    MsmPlan pl = plan(n, batch, stride, off, c, precomp, task_len, chunk);
     MsmLayout<F> L;
     GB_CUDA_TRY(msm_layout<F>(pl, L));
     return msm_enqueue<Fr, F>(st, pl, reinterpret_cast<const Affine<F>*>(d_table),

@@ -42,11 +42,13 @@ struct MsmOps {
   size_t fr_bytes;      // sizeof(fr.Element)
   size_t affine_bytes;  // sizeof(G?Affine)
   size_t jac_bytes;     // sizeof(G?Jac)
-  // workspace bytes for an MSM of n scalars with the given parameters
-  cudaError_t (*ws_bytes)(uint32_t n, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk, size_t* out);
+  // workspace bytes for `batch` MSMs of n scalars each (1: a single MSM) with the given parameters
+  cudaError_t (*ws_bytes)(uint32_t n, uint32_t batch, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk,
+                          size_t* out);
   // enqueue a full MSM (all pointers on device); d_idx null: bases off + i, else bases d_idx[i] (indices checked
-  // against the table's point count by the caller)
-  cudaError_t (*run)(cudaStream_t st, uint32_t n, uint32_t stride, uint32_t off, int c, int precomp,
+  // against the table's point count by the caller).  batch > 1: d_scalars holds batch * n scalars (item-major), d_out_jac
+  // batch points, and d_idx must be null
+  cudaError_t (*run)(cudaStream_t st, uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp,
                      uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars, void* d_out_jac,
                      void* ws, cudaEvent_t* stage_events /* nullable, 8 entries */,
                      const MsmPipe* pipe /* nullable: everything on st */, const uint32_t* d_idx);

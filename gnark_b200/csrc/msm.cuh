@@ -38,6 +38,7 @@ struct MsmPlan {
   uint32_t total_buckets; // nsets * set_size ; also the "no entry" key
   uint32_t task_len;      // max entries per accumulate task
   uint32_t chunk;         // buckets per level-1 reduction chunk
+  uint32_t batch;         // MSMs over the same bases (1 = a single MSM); nsets and total_buckets count every item's sets
 };
 
 HD int msm_num_windows(int scalar_bits, int c) { return scalar_bits / c + 1; }
@@ -53,6 +54,19 @@ HD MsmPlan msm_make_plan(uint32_t n, uint32_t table_stride, uint32_t table_off, 
   p.total_buckets = (uint32_t)p.nsets * p.set_size;
   p.task_len = task_len;
   p.chunk = chunk;
+  p.batch = 1;
+  return p;
+}
+
+// `batch` MSMs of n scalars each over the same bases: one pipeline whose bucket sets are the items' sets side by side
+// (item b owns sets [b * nsets_item, (b + 1) * nsets_item)); sort, offsets, accumulate, combine and the chunk reduction
+// work on any number of contiguous sets and need nothing else
+HD MsmPlan msm_make_batch_plan(uint32_t batch, uint32_t n, uint32_t table_stride, uint32_t table_off, int scalar_bits, int c,
+                               int precomp, uint32_t task_len, uint32_t chunk) {
+  MsmPlan p = msm_make_plan(n, table_stride, table_off, scalar_bits, c, precomp, task_len, chunk);
+  p.batch = batch;
+  p.nsets *= (int)batch;
+  p.total_buckets = (uint32_t)p.nsets * p.set_size;
   return p;
 }
 
@@ -62,14 +76,13 @@ HD MsmPlan msm_make_plan(uint32_t n, uint32_t table_stride, uint32_t table_off, 
 HD bool msm_index_ok(const uint32_t* idx, uint32_t i, uint32_t count) { return idx[i] < count; }
 
 // ---- 1. decompose ----------------------------------------------------------
-// keys/vals are laid out [w][i] (coalesced per window).  val = table index | sign<<31.  The base of scalar i is
-// table_off + i, or idx[i] when an index list is given (checked by msm_index_ok before the MSM is enqueued).
+// Digits of one scalar (Montgomery form) whose base is table index `base`: the entry of window w goes to slot
+// slot0 + w * win_stride, its key lies in bucket set set0 + (precomp ? 0 : w).  val = table index | sign<<31.
 template <class Fr>
-HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint32_t* keys, uint32_t* vals,
-                          const uint32_t* idx = nullptr) {
+HD void msm_decompose_digits(const MsmPlan& pl, const Fr& scalar, uint32_t base, uint32_t set0, size_t slot0,
+                             size_t win_stride, uint32_t* keys, uint32_t* vals) {
   constexpr int N = Fr::N;
-  const Fr s = scalars[i].from_mont();
-  const uint32_t base = idx ? idx[i] : pl.table_off + i;
+  const Fr s = scalar.from_mont();
   uint32_t carry = 0;
   const uint32_t half = pl.set_size;  // 2^(c-1)
   const uint32_t mask = (pl.c == 32) ? 0xffffffffu : ((1u << pl.c) - 1u);
@@ -89,17 +102,35 @@ HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint
       // digit d - 2^c < 0 ; |digit| = 2^c - d  (<= 2^(c-1))
       d = (1u << pl.c) - d; neg = 1; carry = 1;
     }
-    const size_t slot = (size_t)w * pl.n + i;
+    const size_t slot = (size_t)w * win_stride + slot0;
     if (d == 0) {
       keys[slot] = pl.total_buckets;
       vals[slot] = 0;
     } else {
-      const uint32_t set = pl.precomp ? 0u : (uint32_t)w;
+      const uint32_t set = set0 + (pl.precomp ? 0u : (uint32_t)w);
       keys[slot] = set * pl.set_size + (d - 1);
       const uint32_t ti = (pl.precomp ? (uint32_t)w * pl.table_stride : 0u) + base;
       vals[slot] = ti | (neg << 31);
     }
   }
+}
+
+// keys/vals are laid out [w][i] (coalesced per window).  The base of scalar i is table_off + i, or idx[i] when an index
+// list is given (checked by msm_index_ok before the MSM is enqueued).
+template <class Fr>
+HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint32_t* keys, uint32_t* vals,
+                          const uint32_t* idx = nullptr) {
+  msm_decompose_digits<Fr>(pl, scalars[i], idx ? idx[i] : pl.table_off + i, 0u, i, pl.n, keys, vals);
+}
+
+// Batched MSM (msm_make_batch_plan): entry g = b * n + i is scalar i of item b (scalars item-major), base table_off + i
+// as in the single MSM, keys in the item's own sets.  Entries are laid out [w][b][i], so every window stays coalesced;
+// with batch = 1 they are exactly msm_decompose_one's.
+template <class Fr>
+HD void msm_decompose_batch_one(const MsmPlan& pl, uint32_t g, const Fr* scalars, uint32_t* keys, uint32_t* vals) {
+  const uint32_t b = g / pl.n, i = g - b * pl.n;
+  const uint32_t item_sets = (uint32_t)pl.nsets / pl.batch;
+  msm_decompose_digits<Fr>(pl, scalars[g], pl.table_off + i, b * item_sets, g, (size_t)pl.batch * pl.n, keys, vals);
 }
 
 // ---- 3. accumulate ---------------------------------------------------------

@@ -28,6 +28,14 @@ __global__ void __launch_bounds__(256) k_msm_decompose(MsmPlan pl, const Fr* __r
   if (i < pl.n) msm_decompose_one<Fr>(pl, i, scalars, keys, vals, idx);
 }
 
+// batched MSM: one thread per (item, scalar), entry g = b * n + i
+template <class Fr>
+__global__ void __launch_bounds__(256) k_msm_decompose_batch(MsmPlan pl, const Fr* __restrict__ scalars,
+                                                             uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < pl.n * pl.batch) msm_decompose_batch_one<Fr>(pl, g, scalars, keys, vals);
+}
+
 // off[b] = first sorted position with key >= b, for b in [0, nb]
 static __global__ void k_msm_bucket_offsets(const uint32_t* __restrict__ skeys, uint32_t m, uint32_t nb,
                                      uint32_t* __restrict__ off) {
@@ -181,11 +189,19 @@ __global__ void __launch_bounds__(256) k_msm_set_sum(uint32_t chunks_per_set, co
 }
 
 // slice sums -> set sums (warp w takes sets w, w + warps, ...: a 5-level tree over at most 32 slices), then Horner over
-// the sets on one thread; result in gnark Jacobian layout.  set_totals: nsets entries of scratch.
-template <class F>
+// the sets on one thread; result in gnark Jacobian layout.  set_totals: nsets entries of scratch (per block).
+// kBatch: block b finishes MSM b of a batch - its nsets sets follow those of the blocks before it, it writes out[b] - so the
+// items' Horner sums run in parallel.  A single MSM takes the other instantiation, which carries no item offsets (its
+// registers are at the 255 cap on the wide curves, and the offsets would add spills).
+template <class F, bool kBatch>
 __global__ void __launch_bounds__(256) k_msm_finish(int nsets, int c, uint32_t slices, const XYZZ<F>* __restrict__ slice_sums,
                                                     XYZZ<F>* __restrict__ set_totals, Jacobian<F>* __restrict__ out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
+  if (kBatch) {
+    slice_sums += (size_t)blockIdx.x * nsets * slices;
+    set_totals += (size_t)blockIdx.x * nsets;
+    out += blockIdx.x;
+  }
   XYZZ<F>* sm = reinterpret_cast<XYZZ<F>*>(smem_raw) + (threadIdx.x & ~31u);
   const uint32_t lane = threadIdx.x & 31u;
   for (int s = (int)(threadIdx.x >> 5); s < nsets; s += (int)(blockDim.x >> 5)) {
@@ -318,7 +334,7 @@ inline size_t gb_align(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
 template <class F>
 cudaError_t msm_layout(const MsmPlan& pl, MsmLayout<F>& L) {
-  L.m = (size_t)pl.n * pl.nwin;
+  L.m = (size_t)pl.n * pl.batch * pl.nwin;
   L.max_tasks = L.m / pl.task_len + pl.total_buckets + 1;
   L.chunks_per_set = (pl.set_size + pl.chunk - 1) / pl.chunk;
   size_t sort_bytes = 0, scan_bytes = 0;
@@ -355,9 +371,9 @@ inline int msm_set_sum_threads(size_t budget = 160 * 1024) {
   return t;
 }
 
-// Enqueue a full MSM on `stream`.  d_scalars: n Fr elements (Montgomery) on device.
-// d_out: one Jacobian<F> on device.  ws must hold msm_layout().total bytes.  d_idx (optional): n checked table indices,
-// scalar i then multiplies base d_idx[i] instead of base table_off + i.
+// Enqueue a full MSM on `stream`.  d_scalars: n Fr elements (Montgomery) on device; batch * n, item-major, for a plan of
+// msm_make_batch_plan.  d_out: one Jacobian<F> on device per item.  ws must hold msm_layout().total bytes.  d_idx
+// (optional, single MSMs only): n checked table indices, scalar i then multiplies base d_idx[i] instead of base table_off + i.
 template <class Fr, class F>
 cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>* d_table, const Fr* d_scalars,
                         Jacobian<F>* d_out, void* ws, const MsmLayout<F>& L, cudaEvent_t* ev = nullptr,
@@ -386,11 +402,16 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
 
   if (pl.n == 0) {
     // empty sum = infinity
-    k_msm_finish<F><<<1, 32, 32 * sizeof(XYZZ<F>), stream>>>(0, pl.c, 1, sets, sets, d_out);  // nsets = 0: the point at infinity
+    // nsets = 0: the point at infinity
+    if (pl.batch > 1) k_msm_finish<F, true><<<pl.batch, 32, 32 * sizeof(XYZZ<F>), stream>>>(0, pl.c, 1, sets, sets, d_out);
+    else k_msm_finish<F, false><<<1, 32, 32 * sizeof(XYZZ<F>), stream>>>(0, pl.c, 1, sets, sets, d_out);
     return cudaGetLastError();
   }
   GB_EV(0);
-  k_msm_decompose<Fr><<<(pl.n + 255) / 256, 256, 0, stream>>>(pl, d_scalars, keys0, vals0, d_idx);
+  if (pl.batch > 1)
+    k_msm_decompose_batch<Fr><<<(unsigned)((L.m / pl.nwin + 255) / 256), 256, 0, stream>>>(pl, d_scalars, keys0, vals0);
+  else
+    k_msm_decompose<Fr><<<(pl.n + 255) / 256, 256, 0, stream>>>(pl, d_scalars, keys0, vals0, d_idx);
   GB_EV(1);
   int end_bit = 1;
   while ((1ull << end_bit) <= nb) end_bit++;
@@ -436,11 +457,23 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
   if (slices > MSM_SET_SLICES) slices = MSM_SET_SLICES;
   const size_t smem = (size_t)st * sizeof(XYZZ<F>);
   GB_CUDA_TRY(cudaFuncSetAttribute(k_msm_set_sum<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_msm_set_sum<F><<<dim3(slices, (unsigned)pl.nsets), st, smem, stream>>>(L.chunks_per_set, chunks, sets);
-  const int fw = pl.nsets < 8 ? (pl.nsets > 0 ? pl.nsets : 1) : 8;                // warps of the finish block
+  // a grid's y dimension stops at 65535 sets; a large batch of MSMs has more, which go in further launches
+  for (uint32_t s0 = 0; s0 < (uint32_t)pl.nsets; s0 += 65535u) {
+    const uint32_t rows = (uint32_t)pl.nsets - s0 < 65535u ? (uint32_t)pl.nsets - s0 : 65535u;
+    k_msm_set_sum<F><<<dim3(slices, rows), st, smem, stream>>>(L.chunks_per_set, chunks + (size_t)s0 * L.chunks_per_set,
+                                                               sets + (size_t)s0 * slices);
+  }
+  const int item_sets = pl.nsets / (int)pl.batch;
+  const int fw = item_sets < 8 ? (item_sets > 0 ? item_sets : 1) : 8;             // warps of a finish block
   const size_t fsmem = (size_t)fw * 32 * sizeof(XYZZ<F>);
-  GB_CUDA_TRY(cudaFuncSetAttribute(k_msm_finish<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-  k_msm_finish<F><<<1, 32 * fw, fsmem, stream>>>(pl.nsets, pl.c, slices, sets, sets + (size_t)pl.nsets * MSM_SET_SLICES, d_out);
+  XYZZ<F>* set_totals = sets + (size_t)pl.nsets * MSM_SET_SLICES;
+  if (pl.batch > 1) {
+    GB_CUDA_TRY(cudaFuncSetAttribute(k_msm_finish<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    k_msm_finish<F, true><<<pl.batch, 32 * fw, fsmem, stream>>>(item_sets, pl.c, slices, sets, set_totals, d_out);
+  } else {
+    GB_CUDA_TRY(cudaFuncSetAttribute(k_msm_finish<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    k_msm_finish<F, false><<<1, 32 * fw, fsmem, stream>>>(item_sets, pl.c, slices, sets, set_totals, d_out);
+  }
   GB_EV(7);
 #undef GB_EV
   return cudaGetLastError();

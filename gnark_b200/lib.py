@@ -39,7 +39,7 @@ EXPORTS = [
     "b200_comm_unique_id", "b200_comm_init", "b200_comm_init_all", "b200_comm_destroy", "b200_comm_info",
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
-    "b200_points_ntt", "b200_msm_indexed",
+    "b200_points_ntt", "b200_msm_indexed", "b200_msm_batch",
 ]
 COMM_ID_BYTES = 128
 
@@ -158,6 +158,8 @@ def load(path: str = None):
         lib.b200_pedersen_fold.argtypes = [i32, vp, sz, vp, vp]
     if "b200_msm_indexed" not in missing:
         lib.b200_msm_indexed.argtypes = [vp, vp, sz, i32, vp, i32, vp]
+    if "b200_msm_batch" not in missing:
+        lib.b200_msm_batch.argtypes = [vp, sz, sz, sz, vp, i32, vp]
     if "b200_table_upload_encoded" not in missing:
         lib.b200_table_upload_encoded.argtypes = [i32, i32, i32, vp, sz, i32, i32, ctypes.POINTER(vp)]
     if "b200_plonk_set_qk" not in missing:
@@ -407,6 +409,27 @@ class Table:
         out = np.zeros(3 * self.coord_limbs, dtype=np.uint64)
         check(load().b200_msm_indexed(self.handle, ptr(idx), n, 1 if idx_dev else 0, ptr(scalars), 1 if sc_dev else 0,
                                       ptr(out)))
+        return out
+
+    def msm_batch(self, scalars, off: int = 0, n: int = None) -> np.ndarray:
+        """out[b] = sum_i scalars[b, i] * bases[off + i] for every row b: several MSMs over one base range in one call
+        (one pipeline for the whole batch).  scalars: (batch, n, fr_limbs) host array or contiguous device tensor,
+        item-major; n defaults to the row length.  Returns (batch, 3 * coord_limbs) Jacobian points (gnark layout)."""
+        sc_dev = hasattr(scalars, "data_ptr")
+        if sc_dev:
+            if not scalars.is_contiguous():
+                raise ValueError("msm_batch: the device scalars must be contiguous")
+            total = scalars.numel()
+        else:
+            scalars = np.ascontiguousarray(scalars, dtype=np.uint64)
+            total = scalars.size
+        batch = int(scalars.shape[0])
+        if n is None:
+            n = total // (batch * self.fr_limbs) if batch else 0
+        if total != batch * n * self.fr_limbs:
+            raise ValueError(f"msm_batch: {total} scalar words for {batch} rows of {n} scalars")
+        out = np.zeros((batch, 3 * self.coord_limbs), dtype=np.uint64)
+        check(load().b200_msm_batch(self.handle, off, n, batch, ptr(scalars), 1 if sc_dev else 0, ptr(out)))
         return out
 
     def msm_async(self, d_scalars, d_out, off: int = 0, n: int = None):

@@ -348,6 +348,14 @@ func (t *Table) MSMIndexed(idx []uint32, scalars, out unsafe.Pointer) error {
 	return Call(func() int32 { return int32(C.b200_msm_indexed(t.h, ip, C.size_t(len(idx)), 0, scalars, 0, out)) })
 }
 
+// MSMBatch is b200_msm_batch: out[b] = sum_{i<n} scalars[b*n + i] * bases[off + i] for b < batch (batch G?Jac).
+// scalars (batch*n fr.Elements, item-major) and out are host memory borrowed for the call.
+func (t *Table) MSMBatch(off, n, batch int, scalars, out unsafe.Pointer) error {
+	return Call(func() int32 {
+		return int32(C.b200_msm_batch(t.h, C.size_t(off), C.size_t(n), C.size_t(batch), scalars, 0, out))
+	})
+}
+
 // Free is b200_table_free; safe on a nil table and more than once.
 func (t *Table) Free() {
 	if t != nil && t.h != nil {

@@ -188,6 +188,16 @@ int32_t b200_msm_gather(b200_table_t bases, size_t off, const uint32_t* idx, siz
  * names its position and leaves out_jac_host untouched.  n = 0 gives the point at infinity. */
 int32_t b200_msm_indexed(b200_table_t bases, const uint32_t* idx, size_t n, int32_t idx_on_device,
                          const void* scalars_mont, int32_t scalars_on_device, void* out_jac_host);
+/* out[b] = sum_{i<n} scalars[b*n + i] * bases[off + i], b < batch: `batch` MSMs over ONE base range of one table
+ * (ICICLE's BatchSize with ArePointsSharedInBatch).  scalars: batch*n fr.Elements (Montgomery), item-major, host or
+ * device; out_jac_host: batch G?Jac (the table's group) in gnark layout.  The batch runs as one MSM pipeline whose bucket
+ * sets are the items' sets side by side: one sort, one accumulate and one reduction tail for all items.  On a plain table
+ * the window comes from n; a precomputed table keeps the window its slabs were built for.  Limits, checked before anything
+ * is allocated or launched (a violation fails the call, names the limit and leaves out_jac_host untouched):
+ * off + n <= the table's point count, batch * n * windows < 2^31, batch * bucket sets * 2^(c-1) < 2^31 - 1.
+ * batch = 0 writes nothing; n = 0 writes `batch` points at infinity.  Joins pending pipelined MSMs first. */
+int32_t b200_msm_batch(b200_table_t bases, size_t off, size_t n, size_t batch, const void* scalars_mont,
+                       int32_t scalars_on_dev, void* out_jac_host);
 
 /* Pedersen / BSB22 commitment keys (gnark-crypto pedersen.ProvingKey{Basis, BasisExpSigma}, one per commitment:
  * ProvingKey.CommitmentKeys, backend/groth16/bn254/setup.go:46).  b200_pedersen_commit runs
