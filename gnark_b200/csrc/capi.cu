@@ -166,9 +166,17 @@ int msm_window_with_limit(size_t n, int scalar_bits) {
   return c;
 }
 
+size_t msm_max_batch(const b200_table_s* t, size_t n, int c) {
+  const size_t nwin = (size_t)msm_num_windows(t->ops->scalar_bits, c);
+  const size_t by_entries = n ? (((size_t)1 << 31) - 1) / (n * nwin) : SIZE_MAX;
+  const size_t by_keys = (((size_t)1 << 31) - 2) / ((t->precomp ? (size_t)1 : nwin) << (c - 1));
+  return by_entries < by_keys ? by_entries : by_keys;
+}
+
 int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* d_scalars, void* d_out,
-                      cudaEvent_t* stage_events, bool pipelined, const uint32_t* d_idx) {
+                      cudaEvent_t* stage_events, bool pipelined, const uint32_t* d_idx, size_t batch, size_t stride) {
   if (d_idx ? off != 0 : off + n > t->n) return set_error("msm: range [off, off+n) exceeds the table");
+  if (batch > 1 && (d_idx || batch > msm_max_batch(t, n, t->c))) return set_error("msm: batch exceeds the pipeline's indices");
   // a precomputed table's slabs fix its window; an indexed MSM on a plain table sizes its bucket sets by its own n
   // (a few hundred indices into a 2^22-point table must not pay for 2^15-bucket sets)
   const int c = (d_idx && !t->precomp) ? msm_window_with_limit(n, t->ops->scalar_bits) : t->c;
@@ -179,9 +187,9 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
   if (stage_events || n == 0) pipelined = false;
   if (!pipelined) { int32_t rc = msm_join(ctx); if (rc) return rc; }
   uint32_t task_len, chunk;
-  msm_tuning(n, 1, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
+  msm_tuning(n, batch, nwin, c, t->precomp, t->ops->acc_blocks_per_sm(), &task_len, &chunk);
   size_t ws_bytes = 0;
-  CK(t->ops->ws_bytes((uint32_t)n, 1, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
+  CK(t->ops->ws_bytes((uint32_t)n, (uint32_t)batch, (uint32_t)t->n, c, t->precomp, task_len, chunk, &ws_bytes));
   AsyncBuf ws_buf;
   CK(ws_buf.alloc(ws_bytes, ctx->stream));
   void* ws = ws_buf.p;
@@ -197,8 +205,9 @@ int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, con
     pipe.acc_ev = ctx->acc_ev[slot];
     ctx->pipe_seq++;
   }
-  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, 1, (uint32_t)t->n, (uint32_t)off, c, t->precomp, task_len, chunk,
-                              t->d_points, d_scalars, d_out, ws, stage_events, pipelined ? &pipe : nullptr, d_idx);
+  cudaError_t e = t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)batch, (uint32_t)t->n, (uint32_t)off, c, t->precomp,
+                              task_len, chunk, t->d_points, d_scalars, d_out, ws, stage_events, pipelined ? &pipe : nullptr,
+                              d_idx, (uint32_t)stride);
   // the workspace is last used by the tail kernels
   cudaError_t e2 = ws_buf.release_on(pipelined ? ctx->tail_stream : ctx->stream);
   if (pipelined && e == cudaSuccess) {
@@ -683,7 +692,7 @@ int32_t b200_msm_batch(b200_table_t t, size_t off, size_t n, size_t batch, const
   CK(st.scratch(ws_bytes, &ws));
   return st.finish("msm_batch", t->ops->run(ctx->stream, (uint32_t)n, (uint32_t)batch, (uint32_t)t->n, (uint32_t)off, c,
                                             t->precomp, task_len, chunk, t->d_points, sc, d_out, ws, nullptr, nullptr,
-                                            nullptr));
+                                            nullptr, 0));
   GUARD_END
 }
 
@@ -769,6 +778,21 @@ int32_t b200_ntt(b200_domain_t d, void* data, int32_t on_dev, int32_t inverse, i
   void* buf;
   CK(st.inout(data, ((size_t)1 << d->logn) * d->ops->fr_bytes, on_dev, &buf));
   return st.finish("ntt", d->ops->ntt(ctx->stream, d->impl, buf, inverse, decimation, on_coset));
+  GUARD_END
+}
+
+int32_t b200_ntt_batch(b200_domain_t d, void* data, size_t batch, int32_t on_dev, int32_t inverse, int32_t decimation,
+                       int32_t on_coset) {
+  GUARD_BEGIN
+  if (!d) return set_error("ntt_batch: null domain");
+  if (decimation != B200_DIF && decimation != B200_DIT) return set_error("ntt_batch: decimation must be DIF or DIT");
+  if (batch == 0) return 0;
+  if (!data) return set_error("ntt_batch: null data");
+  GB_DEVICE(ctx, d->dev);
+  Staging st(ctx);
+  void* buf;
+  CK(st.inout(data, batch * ((size_t)1 << d->logn) * d->ops->fr_bytes, on_dev, &buf));
+  return st.finish("ntt_batch", d->ops->ntt_batch(ctx->stream, d->impl, buf, batch, inverse, decimation, on_coset));
   GUARD_END
 }
 

@@ -80,8 +80,15 @@ int32_t scratch_alloc(int dev, size_t bytes, void** out);
 int32_t scratch_free(int dev, void* p);
 // d_idx (optional, device): n table indices already checked against t->n; scalar i then multiplies base d_idx[i]
 // (off must be 0).  On a plain table an indexed MSM takes its window from n, not from the table's size.
+// batch > 1: `batch` MSMs over the same bases in one pipeline (msm_make_batch_plan), item b's n scalars at
+// d_scalars + b * stride (0: n), one Jacobian result per item at d_out; the window is the table's, as for a single MSM.
+// The caller checks msm_batch_fits() first.
 int32_t msm_on_stream(DeviceCtx* ctx, b200_table_s* t, size_t off, size_t n, const void* d_scalars, void* d_out,
-                      cudaEvent_t* stage_events = nullptr, bool pipelined = false, const uint32_t* d_idx = nullptr);
+                      cudaEvent_t* stage_events = nullptr, bool pipelined = false, const uint32_t* d_idx = nullptr,
+                      size_t batch = 1, size_t stride = 0);
+// largest batch of n-scalar MSMs with window c on t that the pipeline can index: batch * n * windows entries below 2^31
+// and batch * bucket sets * 2^(c-1) bucket keys below 2^31 - 1 (what b200_msm_batch checks)
+size_t msm_max_batch(const b200_table_s* t, size_t n, int c);
 // window of an MSM of n scalars on a table of `scalar_bits`-bit scalars: msm_window_for(n), raised until the scalar has
 // at most 64 windows (MSM_MAX_WINDOWS of the table precompute)
 int msm_window_with_limit(size_t n, int scalar_bits);

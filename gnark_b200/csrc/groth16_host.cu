@@ -3,6 +3,7 @@
 // Prove :784-1360, computeH :1391-1488) and of the CPU prover
 // backend/groth16/bn254/prove.go:52-315, from "solved witness" to "proof points".
 // The R1CS solver (constraint/bn254/solver.go) stays in Go and is out of scope.
+#include <atomic>
 #include <thread>
 
 #include "capi_common.h"
@@ -225,6 +226,15 @@ static cudaError_t upload_async(cudaStream_t st, void* dst, const void* src, siz
   return cudaSuccess;
 }
 
+// Stream-ordered device buffers of one proof (or one batch of proofs).  Freed on every exit path, early error returns
+// included: the pipelined MSM tails (tail stream) still read and write these buffers, so `st` must wait for them before
+// the stream-ordered frees (and tail_pending must not leak to the next caller).
+struct ProveBufs {
+  DeviceCtx* ctx; cudaStream_t st; std::vector<void*> p;
+  ~ProveBufs() { msm_join(ctx); for (void* q : p) cudaFreeAsync(q, st); }
+  cudaError_t get(void** out, size_t bytes) { cudaError_t e = cudaMallocAsync(out, bytes ? bytes : 1, st); if (e == cudaSuccess) p.push_back(*out); return e; }
+};
+
 static double now_ms() {
   using namespace std::chrono;
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
@@ -254,13 +264,7 @@ int32_t b200_groth16_msms(b200_pk_t pk, const void* wires, const void* a, const 
     return 0;
   };
 
-  struct Bufs {
-    DeviceCtx* ctx; cudaStream_t st; std::vector<void*> p;
-    // every exit path, early error returns included: the pipelined MSM tails (tail stream) still read and write these
-    // buffers, so `st` must wait for them before the stream-ordered frees (and tail_pending must not leak to the next caller)
-    ~Bufs() { msm_join(ctx); for (void* q : p) cudaFreeAsync(q, st); }
-    cudaError_t get(void** out, size_t bytes) { cudaError_t e = cudaMallocAsync(out, bytes ? bytes : 1, st); if (e == cudaSuccess) p.push_back(*out); return e; }
-  } bufs{ctx, st, {}};
+  ProveBufs bufs{ctx, st, {}};
   void *d_w, *d_a, *d_b, *d_c, *d_wa, *d_wb, *d_res;
   CK(bufs.get(&d_w, pk->nb_wires * fb));
   CK(bufs.get(&d_a, n * fb)); CK(bufs.get(&d_b, n * fb)); CK(bufs.get(&d_c, n * fb));
@@ -420,6 +424,144 @@ int32_t b200_groth16_prove(b200_pk_t pk, const void* wires, const void* a, const
   if (msm_out) memcpy(msm_out, msm.data(), msm.size());
   groth16_assemble_with(pk, msm.data(), r, s, d, ar_out, bs_out, krs_out);
   if (getenv("GB200_STEP_PROFILE")) fprintf(stderr, "[gb200 step] %-14s %8.3f ms (device part %.3f ms)\n", "host assembly", now_ms() - t1, t1 - t0);
+  return 0;
+  GUARD_END
+}
+
+}  // extern "C"
+
+namespace {
+// fn(k) for k < count on up to hardware_concurrency host threads; the first exception of a worker is rethrown here
+template <class Fn>
+void parallel_for(size_t count, Fn fn) {
+  size_t threads = std::thread::hardware_concurrency();
+  if (threads == 0) threads = 1;
+  if (threads > count) threads = count;
+  std::atomic<size_t> next{0};
+  std::vector<std::future<void>> workers;
+  for (size_t t = 0; t < threads; t++)
+    workers.push_back(std::async(std::launch::async, [&] { for (size_t k; (k = next++) < count;) fn(k); }));
+  for (auto& w : workers) w.get();
+}
+
+// Device part of b200_groth16_prove_batch: the launch sequence of b200_groth16_msms with every stage over the whole
+// batch - the wires of all items go up and are filtered in one launch per filter, each table's MSM is one batched MSM
+// (pipelined like the single proof's five), A, B, C of all items go up on the copy stream into one [3][batch][n]
+// buffer whose computeH runs as batched NTTs.  msm_out: the five tables' results table-major, [A | B1 | Z | K][batch]
+// G1 Jacobians, then [batch] G2 Jacobians of B2.
+int32_t groth16_msms_batch(DeviceCtx* ctx, b200_pk_t pk, size_t batch, const void* const* wires, const void* const* a,
+                           const void* const* b, const void* const* c, size_t n_constraints, void* msm_out) {
+  cudaStream_t st = ctx->stream;
+  const size_t fb = pk->fr->fr_bytes, n = pk->n, nw = pk->nb_wires;
+  const size_t j1 = pk->h1->jac_bytes, j2 = pk->h2->jac_bytes;
+  ProveBufs bufs{ctx, st, {}};
+  void *d_w, *d_abc, *d_wa, *d_wb, *d_res;
+  CK(bufs.get(&d_w, batch * nw * fb));
+  CK(bufs.get(&d_abc, 3 * batch * n * fb));
+  CK(bufs.get(&d_wa, batch * pk->n_a * fb));
+  CK(bufs.get(&d_wb, batch * pk->n_b * fb));
+  CK(bufs.get(&d_res, batch * (4 * j1 + j2)));
+  char* w = static_cast<char*>(d_w);
+  for (size_t k = 0; k < batch; k++) CK(upload_async(st, w + k * nw * fb, wires[k], nw * fb));
+  CK(pk->fr->gather_batch(st, d_wa, d_w, pk->d_idx_a, pk->n_a, batch, nw, pk->n_a));
+  CK(pk->fr->gather_batch(st, d_wb, d_w, pk->d_idx_b, pk->n_b, batch, nw, pk->n_b));
+  char* res = static_cast<char*>(d_res);
+  auto out = [&](int table) { return res + (size_t)table * batch * j1; };
+  int32_t rc = msm_on_stream(ctx, pk->A, 0, pk->n_a, d_wa, out(0), nullptr, true, nullptr, batch, pk->n_a);
+  if (rc) return rc;
+  rc = msm_on_stream(ctx, pk->B1, 0, pk->n_b, d_wb, out(1), nullptr, true, nullptr, batch, pk->n_b);
+  if (rc) return rc;
+  const void* k_scalars = w + pk->nb_public * fb;     // the private tail of each wire vector (keys are not sharded here)
+  size_t k_stride = nw;
+  if (pk->d_idx_k) {
+    void* d_wk;
+    CK(bufs.get(&d_wk, batch * pk->cnt_k * fb));
+    CK(pk->fr->gather_batch(st, d_wk, d_w, pk->d_idx_k, pk->cnt_k, batch, nw, pk->cnt_k));
+    k_scalars = d_wk;
+    k_stride = pk->cnt_k;
+  }
+  rc = msm_on_stream(ctx, pk->K, 0, pk->cnt_k, k_scalars, out(3), nullptr, true, nullptr, batch, k_stride);
+  if (rc) return rc;
+  rc = msm_on_stream(ctx, pk->B2, 0, pk->n_b, d_wb, out(4), nullptr, true, nullptr, batch, pk->n_b);
+  if (rc) return rc;
+  // A, B, C of every item on the copy stream while the four h-independent MSMs run
+  cudaStream_t cs = ctx->copy_stream;
+  CK(cudaEventRecord(ctx->copy_ev, st));            // d_abc was allocated in st's order
+  CK(cudaStreamWaitEvent(cs, ctx->copy_ev, 0));
+  const void* const* src[3] = {a, b, c};
+  char* abc = static_cast<char*>(d_abc);
+  for (int m = 0; m < 3; m++)
+    for (size_t k = 0; k < batch; k++) {
+      char* dst = abc + (m * batch + k) * n * fb;
+      if (n_constraints) CK(upload_async(cs, dst, src[m][k], n_constraints * fb));
+      if (n_constraints < n) CK(cudaMemsetAsync(dst + n_constraints * fb, 0, (n - n_constraints) * fb, cs));
+    }
+  CK(cudaEventRecord(ctx->copy_ev, cs));
+  CK(cudaStreamWaitEvent(st, ctx->copy_ev, 0));
+  CK(pk->fr->compute_h_batch(st, pk->dom->impl, d_abc, batch));
+  // Z over the first n - 1 elements of each item's h
+  rc = msm_on_stream(ctx, pk->Z, 0, pk->cnt_z, d_abc, out(2), nullptr, true, nullptr, batch, n);
+  if (rc) return rc;
+  rc = msm_join(ctx);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(msm_out, d_res, batch * (4 * j1 + j2), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int32_t b200_groth16_prove_batch(b200_pk_t pk, size_t batch, const void* const* wires, const void* const* a,
+                                 const void* const* b, const void* const* c, size_t n_constraints, const void* r,
+                                 const void* s, void* ar_out, void* bs_out, void* krs_out, void* msm_out) {
+  GUARD_BEGIN
+  if (!pk) return set_error("prove_batch: null proving key");
+  if (pk->shard_world > 1)
+    return set_error("prove_batch: sharded keys are not supported - prove each proof with b200_groth16_prove");
+  if (n_constraints > pk->n) return set_error("prove_batch: more constraints than the domain holds");
+  if (batch == 0) return 0;
+  if (!wires || !a || !b || !c || !r || !s || !ar_out || !bs_out || !krs_out) return set_error("prove_batch: null argument");
+  // every index the batch needs fits its device counters: the five batched MSMs (2^31 entries, 2^31 - 1 bucket keys,
+  // each at the window of the table's single MSM) and the 32-bit element indices of the pointwise and gather kernels
+  const size_t n = pk->n, nw = pk->nb_wires;
+  size_t fits = (((size_t)1 << 32) - 1) / (n > nw ? n : (nw ? nw : 1));
+  const std::pair<b200_table_s*, size_t> tables[5] = {{pk->A, pk->n_a}, {pk->B1, pk->n_b}, {pk->Z, pk->cnt_z},
+                                                      {pk->K, pk->cnt_k}, {pk->B2, pk->n_b}};
+  for (const auto& t : tables) {
+    const size_t m = msm_max_batch(t.first, t.second, t.first->c);
+    if (m < fits) fits = m;
+  }
+  if (batch > fits)
+    return set_error("prove_batch: a batch of " + std::to_string(batch) + " proofs exceeds the device indices (2^31 MSM "
+                     "entries and bucket keys per table, 2^32 elements per batched vector) - the largest batch this key "
+                     "takes is " + std::to_string(fits));
+  for (size_t k = 0; k < batch; k++)
+    if (!wires[k] || !a[k] || !b[k] || !c[k]) return set_error("prove_batch: null witness vector of item " + std::to_string(k));
+  GB_DEVICE(ctx, pk->dev);
+  const HostGroupOps* h1 = pk->h1;
+  const HostGroupOps* h2 = pk->h2;
+  const size_t fb = pk->fr->fr_bytes, j1 = h1->jac_bytes, j2 = h2->jac_bytes;
+  auto item = [](const void* p, size_t k, size_t bytes) { return static_cast<const char*>(p) + k * bytes; };
+  // the delta multiples of every item (prove.go:185) on host threads, under the device work
+  std::vector<Groth16Deltas> deltas(batch);
+  std::future<void> dfut = std::async(std::launch::async, [&] {
+    parallel_for(batch, [&](size_t k) { deltas[k] = groth16_deltas(pk, item(r, k, fb), item(s, k, fb)); });
+  });
+  std::vector<uint8_t> msm(batch * (4 * j1 + j2));
+  const int32_t rc = groth16_msms_batch(ctx, pk, batch, wires, a, b, c, n_constraints, msm.data());
+  dfut.get();                                   // joined on every path: the workers read pk, r, s
+  if (rc) return rc;
+  parallel_for(batch, [&](size_t k) {
+    // item k's five results in b200_groth16_prove's layout
+    std::vector<uint8_t> m5(4 * j1 + j2);
+    for (int t = 0; t < 4; t++) memcpy(m5.data() + t * j1, msm.data() + ((size_t)t * batch + k) * j1, j1);
+    memcpy(m5.data() + 4 * j1, msm.data() + 4 * batch * j1 + k * j2, j2);
+    if (msm_out) memcpy(static_cast<char*>(msm_out) + k * m5.size(), m5.data(), m5.size());
+    groth16_assemble_with(pk, m5.data(), item(r, k, fb), item(s, k, fb), deltas[k],
+                          static_cast<char*>(ar_out) + k * h1->affine_bytes, static_cast<char*>(bs_out) + k * h2->affine_bytes,
+                          static_cast<char*>(krs_out) + k * h1->affine_bytes);
+  });
   return 0;
   GUARD_END
 }

@@ -18,8 +18,9 @@ namespace gb200 {
 template <class Fr, class F>
 struct MsmInst {
   static MsmPlan plan(uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp, uint32_t task_len,
-                      uint32_t chunk) {
-    return msm_make_batch_plan(batch, n, stride, off, Fr::Params::BITS, c, precomp, task_len, chunk);   // batch 1: msm_make_plan's
+                      uint32_t chunk, uint32_t scalar_stride = 0) {
+    // batch 1: msm_make_plan's
+    return msm_make_batch_plan(batch, n, stride, off, Fr::Params::BITS, c, precomp, task_len, chunk, scalar_stride);
   }
   static cudaError_t ws_bytes(uint32_t n, uint32_t batch, uint32_t stride, int c, int precomp, uint32_t task_len, uint32_t chunk,
                               size_t* out) {
@@ -31,8 +32,9 @@ struct MsmInst {
   }
   static cudaError_t run(cudaStream_t st, uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp,
                          uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars,
-                         void* d_out_jac, void* ws, cudaEvent_t* ev, const MsmPipe* pipe, const uint32_t* d_idx) {
-    MsmPlan pl = plan(n, batch, stride, off, c, precomp, task_len, chunk);
+                         void* d_out_jac, void* ws, cudaEvent_t* ev, const MsmPipe* pipe, const uint32_t* d_idx,
+                         uint32_t scalar_stride) {
+    MsmPlan pl = plan(n, batch, stride, off, c, precomp, task_len, chunk, scalar_stride);
     MsmLayout<F> L;
     GB_CUDA_TRY(msm_layout<F>(pl, L));
     return msm_enqueue<Fr, F>(st, pl, reinterpret_cast<const Affine<F>*>(d_table),
@@ -141,6 +143,15 @@ __global__ void __launch_bounds__(256) k_gather(Fr* __restrict__ out, const Fr* 
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = src[idx[i]];
 }
+// the same filter over a batch of source vectors: blockIdx.y is the item, out[b * out_stride + j] = src[b * src_stride +
+// idx[j]]; 32-bit element indices (the caller keeps batch * src_stride and batch * out_stride below 2^32)
+template <class Fr>
+__global__ void __launch_bounds__(256) k_gather_batch(Fr* __restrict__ out, const Fr* __restrict__ src,
+                                                      const uint32_t* __restrict__ idx, uint32_t n, uint32_t src_stride,
+                                                      uint32_t out_stride) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) out[blockIdx.y * out_stride + j] = src[blockIdx.y * src_stride + idx[j]];
+}
 
 // ---------------------------------------------------------------------------
 // NTT
@@ -159,6 +170,14 @@ struct NttInst {
   static cudaError_t ntt(cudaStream_t st, void* dom, void* data, int inverse, int decimation, int on_coset) {
     return ntt_enqueue<Fr>(st, *reinterpret_cast<Dom*>(dom), reinterpret_cast<Fr*>(data), inverse != 0, decimation,
                            on_coset != 0);
+  }
+  static cudaError_t ntt_batch(cudaStream_t st, void* dom, void* data, size_t batch, int inverse, int decimation,
+                               int on_coset) {
+    return ntt_enqueue<Fr>(st, *reinterpret_cast<Dom*>(dom), reinterpret_cast<Fr*>(data), inverse != 0, decimation,
+                           on_coset != 0, batch);
+  }
+  static cudaError_t compute_h_batch(cudaStream_t st, void* dom, void* abc, size_t batch) {
+    return compute_h_batch_enqueue<Fr>(st, *reinterpret_cast<Dom*>(dom), reinterpret_cast<Fr*>(abc), batch);
   }
   static cudaError_t compute_h(cudaStream_t st, void* dom, void* a, void* b, void* c) {
     return compute_h_enqueue<Fr>(st, *reinterpret_cast<Dom*>(dom), reinterpret_cast<Fr*>(a), reinterpret_cast<Fr*>(b),
@@ -364,6 +383,18 @@ struct NttInst {
     k_gather<Fr><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((Fr*)out, (const Fr*)src, idx, n);
     return cudaGetLastError();
   }
+  static cudaError_t gather_batch(cudaStream_t st, void* out, const void* src, const uint32_t* idx, size_t n, size_t batch,
+                                  size_t src_stride, size_t out_stride) {
+    if (!n || !batch) return cudaSuccess;
+    for (size_t b0 = 0; b0 < batch; b0 += NTT_MAX_GRID_Y) {     // the y dimension's limit, as for the NTT
+      const unsigned rows = (unsigned)(batch - b0 < NTT_MAX_GRID_Y ? batch - b0 : NTT_MAX_GRID_Y);
+      k_gather_batch<Fr><<<dim3((unsigned)((n + 255) / 256), rows), 256, 0, st>>>(
+          (Fr*)out + b0 * out_stride, (const Fr*)src + b0 * src_stride, idx, (uint32_t)n, (uint32_t)src_stride,
+          (uint32_t)out_stride);
+      GB_CUDA_TRY(cudaGetLastError());
+    }
+    return cudaSuccess;
+  }
   static const HostFrCtx* host_fr() {
     static const HostFrCtx c = HostFrCtx::make<typename Fr::Params>();
     return &c;
@@ -372,7 +403,7 @@ struct NttInst {
     static const NttOps o = {sizeof(Fr), Fr::Params::TWO_ADICITY, &domain_new, &domain_free, &domain_bytes, &ntt,
                              &compute_h, &vec_op, &bit_reverse, &scale_powers, &batch_invert, &plonk_coset,
                              &plonk_divide_by_zh, &axpy, &scan, &plonk_build_z, &poly_eval, &poly_div_linear, &gather,
-                             &host_fr, &plonk_bsb22};
+                             &host_fr, &plonk_bsb22, &ntt_batch, &compute_h_batch, &gather_batch};
     return &o;
   }
 };

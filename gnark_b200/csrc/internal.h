@@ -48,10 +48,11 @@ struct MsmOps {
   // enqueue a full MSM (all pointers on device); d_idx null: bases off + i, else bases d_idx[i] (indices checked
   // against the table's point count by the caller).  batch > 1: d_scalars holds batch * n scalars (item-major), d_out_jac
   // batch points, and d_idx must be null
+  // item b's scalars start at d_scalars + b * scalar_stride (0: n, the items back to back)
   cudaError_t (*run)(cudaStream_t st, uint32_t n, uint32_t batch, uint32_t stride, uint32_t off, int c, int precomp,
                      uint32_t task_len, uint32_t chunk, const void* d_table, const void* d_scalars, void* d_out_jac,
                      void* ws, cudaEvent_t* stage_events /* nullable, 8 entries */,
-                     const MsmPipe* pipe /* nullable: everything on st */, const uint32_t* d_idx);
+                     const MsmPipe* pipe /* nullable: everything on st */, const uint32_t* d_idx, uint32_t scalar_stride);
   // fill slabs 1..nwin-1 of a [nwin][n] table whose slab 0 holds the bases
   cudaError_t (*precompute)(cudaStream_t st, uint32_t n, int nwin, int c, void* d_table);
   // resident 128-thread blocks of the accumulate kernel per SM (occupancy API): the task length is chosen so that the
@@ -102,6 +103,13 @@ struct NttOps {
   // BSB22 commitment gate: out[scatter(j)] += qcp[j] * pi2[j] on one coset (plonk.cuh)
   cudaError_t (*plonk_bsb22)(cudaStream_t st, void* dom0, const void* d_qcp, const void* d_pi2, uint32_t coset_index,
                              uint32_t rho, void* d_out);
+  // `batch` transforms of the domain's size on batch * n item-major elements (ntt_enqueue with a batch)
+  cudaError_t (*ntt_batch)(cudaStream_t st, void* dom, void* d_data, size_t batch, int inverse, int decimation, int on_coset);
+  // computeH of `batch` proofs: d_abc is [3][batch][n] (A, B, C); h of item b ends at d_abc + b * n (compute_h_batch_enqueue)
+  cudaError_t (*compute_h_batch)(cudaStream_t st, void* dom, void* d_abc, size_t batch);
+  // gather over a batch: out[b * out_stride + j] = src[b * src_stride + idx[j]], j < n, b < batch
+  cudaError_t (*gather_batch)(cudaStream_t st, void* d_out, const void* d_src, const uint32_t* d_idx, size_t n, size_t batch,
+                              size_t src_stride, size_t out_stride);
 };
 
 // Host-side group arithmetic for proof assembly (backend/groth16/bn254/prove.go:

@@ -39,6 +39,7 @@ struct MsmPlan {
   uint32_t task_len;      // max entries per accumulate task
   uint32_t chunk;         // buckets per level-1 reduction chunk
   uint32_t batch;         // MSMs over the same bases (1 = a single MSM); nsets and total_buckets count every item's sets
+  uint32_t scalar_stride; // batch: scalars between the first scalars of consecutive items (>= n)
 };
 
 HD int msm_num_windows(int scalar_bits, int c) { return scalar_bits / c + 1; }
@@ -55,16 +56,20 @@ HD MsmPlan msm_make_plan(uint32_t n, uint32_t table_stride, uint32_t table_off, 
   p.task_len = task_len;
   p.chunk = chunk;
   p.batch = 1;
+  p.scalar_stride = n;
   return p;
 }
 
 // `batch` MSMs of n scalars each over the same bases: one pipeline whose bucket sets are the items' sets side by side
 // (item b owns sets [b * nsets_item, (b + 1) * nsets_item)); sort, offsets, accumulate, combine and the chunk reduction
-// work on any number of contiguous sets and need nothing else
+// work on any number of contiguous sets and need nothing else.  Item b's scalars start at scalar b * scalar_stride, so
+// the items can be the first n elements of longer vectors (the n - 1 of an n-long h, the tail of a wire vector);
+// 0 stands for n (items back to back).
 HD MsmPlan msm_make_batch_plan(uint32_t batch, uint32_t n, uint32_t table_stride, uint32_t table_off, int scalar_bits, int c,
-                               int precomp, uint32_t task_len, uint32_t chunk) {
+                               int precomp, uint32_t task_len, uint32_t chunk, uint32_t scalar_stride = 0) {
   MsmPlan p = msm_make_plan(n, table_stride, table_off, scalar_bits, c, precomp, task_len, chunk);
   p.batch = batch;
+  p.scalar_stride = scalar_stride ? scalar_stride : n;
   p.nsets *= (int)batch;
   p.total_buckets = (uint32_t)p.nsets * p.set_size;
   return p;
@@ -123,14 +128,15 @@ HD void msm_decompose_one(const MsmPlan& pl, uint32_t i, const Fr* scalars, uint
   msm_decompose_digits<Fr>(pl, scalars[i], idx ? idx[i] : pl.table_off + i, 0u, i, pl.n, keys, vals);
 }
 
-// Batched MSM (msm_make_batch_plan): entry g = b * n + i is scalar i of item b (scalars item-major), base table_off + i
-// as in the single MSM, keys in the item's own sets.  Entries are laid out [w][b][i], so every window stays coalesced;
-// with batch = 1 they are exactly msm_decompose_one's.
+// Batched MSM (msm_make_batch_plan): entry g = b * n + i is scalar i of item b, read at b * scalar_stride + i (32-bit:
+// the caller keeps batch * scalar_stride below 2^32), base table_off + i as in the single MSM, keys in the item's own sets.
+// Entries are laid out [w][b][i], so every window stays coalesced; with batch = 1 they are exactly msm_decompose_one's.
 template <class Fr>
 HD void msm_decompose_batch_one(const MsmPlan& pl, uint32_t g, const Fr* scalars, uint32_t* keys, uint32_t* vals) {
   const uint32_t b = g / pl.n, i = g - b * pl.n;
   const uint32_t item_sets = (uint32_t)pl.nsets / pl.batch;
-  msm_decompose_digits<Fr>(pl, scalars[g], pl.table_off + i, b * item_sets, g, (size_t)pl.batch * pl.n, keys, vals);
+  msm_decompose_digits<Fr>(pl, scalars[b * pl.scalar_stride + i], pl.table_off + i, b * item_sets, g, (size_t)pl.batch * pl.n,
+                           keys, vals);
 }
 
 // ---- 3. accumulate ---------------------------------------------------------

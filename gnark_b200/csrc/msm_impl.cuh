@@ -28,11 +28,13 @@ __global__ void __launch_bounds__(256) k_msm_decompose(MsmPlan pl, const Fr* __r
   if (i < pl.n) msm_decompose_one<Fr>(pl, i, scalars, keys, vals, idx);
 }
 
-// batched MSM: one thread per (item, scalar), entry g = b * n + i
-template <class Fr>
+// batched MSM: one thread per (item, scalar), entry g = b * n + i.  kStrided = false: the items' scalars are back to back
+// (scalar_stride = n), the index folds to g and the kernel keeps the registers of the unstrided read
+template <class Fr, bool kStrided>
 __global__ void __launch_bounds__(256) k_msm_decompose_batch(MsmPlan pl, const Fr* __restrict__ scalars,
                                                              uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
   const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (!kStrided) pl.scalar_stride = pl.n;
   if (g < pl.n * pl.batch) msm_decompose_batch_one<Fr>(pl, g, scalars, keys, vals);
 }
 
@@ -408,8 +410,10 @@ cudaError_t msm_enqueue(cudaStream_t stream, const MsmPlan& pl, const Affine<F>*
     return cudaGetLastError();
   }
   GB_EV(0);
-  if (pl.batch > 1)
-    k_msm_decompose_batch<Fr><<<(unsigned)((L.m / pl.nwin + 255) / 256), 256, 0, stream>>>(pl, d_scalars, keys0, vals0);
+  if (pl.batch > 1 && pl.scalar_stride != pl.n)
+    k_msm_decompose_batch<Fr, true><<<(unsigned)((L.m / pl.nwin + 255) / 256), 256, 0, stream>>>(pl, d_scalars, keys0, vals0);
+  else if (pl.batch > 1)
+    k_msm_decompose_batch<Fr, false><<<(unsigned)((L.m / pl.nwin + 255) / 256), 256, 0, stream>>>(pl, d_scalars, keys0, vals0);
   else
     k_msm_decompose<Fr><<<(pl.n + 255) / 256, 256, 0, stream>>>(pl, d_scalars, keys0, vals0, d_idx);
   GB_EV(1);

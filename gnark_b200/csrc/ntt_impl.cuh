@@ -40,8 +40,10 @@ __device__ __forceinline__ Fr ntt_ldg(const Fr* __restrict__ p) {
   return v;
 }
 
-// One pass: tile of 2^(S+cb) elements in shared memory (limb-major), blockDim = tile/2.
-template <class Fr>
+// One pass: tile of 2^(S+cb) elements in shared memory (limb-major), blockDim = tile/2.  kBatch: blockIdx.y selects the
+// vector of a batch (vector b at data + b * 2^logn); tables and the pre / post indices are those of the vector.  A single
+// transform takes the other instantiation, whose registers the vector offset would raise (BN254: 62 -> 64, the cap).
+template <class Fr, bool kBatch>
 __global__ void __launch_bounds__(1 << (NTT_MAX_TILE_LOG - 1))
 k_ntt_pass(NttPass p, int logn, int dit, const Fr* __restrict__ tw, Fr* __restrict__ data,
                            const Fr* __restrict__ pre, int pre_bitrev, const Fr* __restrict__ post, int post_bitrev,
@@ -52,6 +54,7 @@ k_ntt_pass(NttPass p, int logn, int dit, const Fr* __restrict__ tw, Fr* __restri
   const uint32_t half = tile_elems >> 1;
   const uint32_t t = threadIdx.x;
   const uint32_t tile = blockIdx.x;
+  if (kBatch) data += (size_t)blockIdx.y << logn;
 
   // load (+ optional pre-scale)
 #pragma unroll
@@ -104,9 +107,12 @@ k_ntt_pass(NttPass p, int logn, int dit, const Fr* __restrict__ tw, Fr* __restri
   }
 }
 
-// n == 1 degenerate transform: only scaling applies
+// n == 1 degenerate transform: only scaling applies, to each of the `batch` one-element vectors
 template <class Fr>
-__global__ void k_ntt_scale1(Fr* data, Fr c) { if (threadIdx.x == 0 && blockIdx.x == 0) data[0] = data[0] * c; }
+__global__ void __launch_bounds__(256) k_ntt_scale1(Fr* data, Fr c, size_t batch) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < batch) data[i] = data[i] * c;
+}
 
 template <class Fr>
 struct NttDomainDev {
@@ -179,15 +185,21 @@ struct NttDomainDev {
   }
 };
 
-// Enqueue one transform, in place on device data (n elements).
-//   extra_pre : optional table multiplied in at load of the first pass (natural index)
+// a grid's y dimension stops at 65535: larger batches of vectors go in further launches
+constexpr size_t NTT_MAX_GRID_Y = 65535;
+
+// Enqueue `batch` transforms, in place on device data (batch * n elements, vector b at data + b * n).
 template <class Fr>
 cudaError_t ntt_enqueue(cudaStream_t st, const NttDomainDev<Fr>& d, Fr* data, bool inverse, int decimation,
-                        bool on_coset) {
+                        bool on_coset, size_t batch = 1) {
   const Fr* T = inverse ? d.itw : d.tw;
   const bool dit = decimation == NTT_DIT;
+  if (batch == 0) return cudaSuccess;
   if (d.logn == 0) {
-    if (inverse) { k_ntt_scale1<Fr><<<1, 1, 0, st>>>(data, d.ninv); }
+    if (inverse) {
+      const size_t threads = batch < 256 ? batch : 256;
+      k_ntt_scale1<Fr><<<(unsigned)((batch + threads - 1) / threads), (unsigned)threads, 0, st>>>(data, d.ninv, batch);
+    }
     return cudaGetLastError();
   }
   for (int pi = 0; pi < d.plan.npasses; pi++) {
@@ -203,20 +215,40 @@ cudaError_t ntt_enqueue(cudaStream_t st, const NttDomainDev<Fr>& d, Fr* data, bo
     const uint32_t tile_elems = 1u << (p.S + p.cb);
     const uint32_t ntiles = d.n >> (p.S + p.cb);
     const size_t smem = (size_t)tile_elems * sizeof(Fr);
-    GB_CUDA_TRY(cudaFuncSetAttribute(k_ntt_pass<Fr>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(NTT_MAX_TILE_LOG >= 11 ? (sizeof(Fr) << NTT_MAX_TILE_LOG) : smem)));
-    k_ntt_pass<Fr><<<ntiles, tile_elems / 2, smem, st>>>(p, d.logn, dit ? 1 : 0, T, data, pre, pre_br, post, post_br,
-                                                        use_const, d.ninv);
-    GB_CUDA_TRY(cudaGetLastError());
+    const int max_smem = (int)(NTT_MAX_TILE_LOG >= 11 ? (sizeof(Fr) << NTT_MAX_TILE_LOG) : smem);
+    if (batch == 1) {
+      GB_CUDA_TRY(cudaFuncSetAttribute(k_ntt_pass<Fr, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+      k_ntt_pass<Fr, false><<<ntiles, tile_elems / 2, smem, st>>>(p, d.logn, dit ? 1 : 0, T, data, pre, pre_br, post, post_br,
+                                                                  use_const, d.ninv);
+      GB_CUDA_TRY(cudaGetLastError());
+      continue;
+    }
+    GB_CUDA_TRY(cudaFuncSetAttribute(k_ntt_pass<Fr, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    for (size_t b0 = 0; b0 < batch; b0 += NTT_MAX_GRID_Y) {
+      const unsigned rows = (unsigned)(batch - b0 < NTT_MAX_GRID_Y ? batch - b0 : NTT_MAX_GRID_Y);
+      k_ntt_pass<Fr, true><<<dim3(ntiles, rows), tile_elems / 2, smem, st>>>(p, d.logn, dit ? 1 : 0, T, data + b0 * d.n, pre,
+                                                                             pre_br, post, post_br, use_const, d.ninv);
+      GB_CUDA_TRY(cudaGetLastError());
+    }
   }
   return cudaSuccess;
 }
 
 // a[i] = (a[i]*b[i] - c[i]) * den      (prove.go:377-383; ICICLE: 3 VecOps icicle.go:1455-1461)
+// (the batched computeH runs it over the k * n elements of the k items' a, b and c)
 template <class Fr>
 __global__ void __launch_bounds__(256) k_h_pointwise(uint32_t n, Fr* __restrict__ a, const Fr* __restrict__ b,
                                                      const Fr* __restrict__ c, Fr den) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) a[i] = (a[i] * b[i] - c[i]) * den;
+}
+
+// 1 / (g^n - 1) of the coset g: the vanishing polynomial's inverse on the coset
+template <class Fr>
+Fr compute_h_den(const NttDomainDev<Fr>& d) {
+  Fr gn = d.coset;
+  for (int k = 0; k < d.logn; k++) gn = gn.sqr();
+  return (gn - Fr::one()).inverse();
 }
 
 // computeH on device.  a, b, c: n-element device vectors (already zero padded);
@@ -228,13 +260,23 @@ cudaError_t compute_h_enqueue(cudaStream_t st, const NttDomainDev<Fr>& d, Fr* a,
     GB_CUDA_TRY(ntt_enqueue<Fr>(st, d, v[k], true, NTT_DIF, false));
     GB_CUDA_TRY(ntt_enqueue<Fr>(st, d, v[k], false, NTT_DIT, true));
   }
-  // den = 1 / (g^n - 1)
-  Fr gn = d.coset;
-  for (int k = 0; k < d.logn; k++) gn = gn.sqr();
-  Fr den = (gn - Fr::one()).inverse();
-  k_h_pointwise<Fr><<<(d.n + 255) / 256, 256, 0, st>>>(d.n, a, b, c, den);
+  k_h_pointwise<Fr><<<(d.n + 255) / 256, 256, 0, st>>>(d.n, a, b, c, compute_h_den(d));
   GB_CUDA_TRY(cudaGetLastError());
   return ntt_enqueue<Fr>(st, d, a, true, NTT_DIF, true);
+}
+
+// computeH of `batch` proofs on one domain.  abc: [3][batch][n] device vectors (A of every item, then B, then C,
+// already zero padded); on return h of item b is at abc + b * n, bit-reversed, exactly as compute_h_enqueue leaves a.
+// batch * n must fit the pointwise kernel's 32-bit index (checked by the caller).
+template <class Fr>
+cudaError_t compute_h_batch_enqueue(cudaStream_t st, const NttDomainDev<Fr>& d, Fr* abc, size_t batch) {
+  if (batch == 0) return cudaSuccess;
+  GB_CUDA_TRY(ntt_enqueue<Fr>(st, d, abc, true, NTT_DIF, false, 3 * batch));
+  GB_CUDA_TRY(ntt_enqueue<Fr>(st, d, abc, false, NTT_DIT, true, 3 * batch));
+  const uint32_t kn = (uint32_t)(batch * d.n);
+  k_h_pointwise<Fr><<<(kn + 255) / 256, 256, 0, st>>>(kn, abc, abc + (size_t)kn, abc + 2 * (size_t)kn, compute_h_den(d));
+  GB_CUDA_TRY(cudaGetLastError());
+  return ntt_enqueue<Fr>(st, d, abc, true, NTT_DIF, true, batch);
 }
 
 }  // namespace gb200

@@ -347,6 +347,46 @@ def ProveSolution(pk: ProvingKey, sol: R1CSSolution, *opts: Option, keep_msm: bo
     return Proof(Ar=ar, Bs=bs, Krs=krs, msm=msm if keep_msm else None)
 
 
+def ProveSolutionBatch(pk: ProvingKey, sols, *opts: Option, keep_msm: bool = False) -> List[Proof]:
+    """Several proofs of one circuit in one call (b200_groth16_prove_batch): the device work of all of them runs as one
+    launch sequence, so small proofs stop paying the fixed cost of an MSM and an NTT pipeline each.  Proof k equals
+    ProveSolution(pk, sols[k]) with the same r, s; the randomness is drawn r0, s0, r1, s1, ...  One device only."""
+    cfg = NewConfig(*opts)
+    if len(cfg.Devices) > 1 or cfg.ShardWorld > 1:
+        raise ValueError("ProveSolutionBatch: one device and an unsharded key only (WithDevices / WithSharding)")
+    sols = list(sols)
+    frl, fpl, deg = _lib.CURVE_SHAPES[pk.curve]
+    for sol in sols:
+        if sol.W.size // frl != pk.nb_wires:
+            raise ValueError("witness size does not match the proving key")
+    n_constraints = sols[0].A.size // frl if sols else 0
+    if any(x.size // frl != n_constraints for sol in sols for x in (sol.A, sol.B, sol.C)):
+        raise ValueError("ProveSolutionBatch: the solutions have different constraint counts (one circuit per batch)")
+    if not sols:
+        return []
+    pk.setup_device_pointers(cfg)
+    q = _FR_MODULUS[pk.curve]
+    rnd = cfg.Randomness or (lambda modulus: secrets.randbelow(modulus))
+    rs = np.stack([_fr_to_mont_limbs(rnd(q), pk.curve) for _ in range(2 * len(sols))])
+    r, s = np.ascontiguousarray(rs[0::2]), np.ascontiguousarray(rs[1::2])
+    k = len(sols)
+    vecs = {name: [np.ascontiguousarray(getattr(sol, name), dtype=np.uint64) for sol in sols] for name in "WABC"}
+    arrays = {name: (ctypes.c_void_p * k)(*[v.ctypes.data for v in vs]) for name, vs in vecs.items()}
+    ar = np.zeros((k, 2 * fpl), dtype=np.uint64)
+    krs = np.zeros((k, 2 * fpl), dtype=np.uint64)
+    bs = np.zeros((k, 2 * fpl * deg), dtype=np.uint64)
+    msm = np.zeros((k, 4 * 3 * fpl + 3 * fpl * deg), dtype=np.uint64) if keep_msm else None
+    p = _lib.ptr
+    _lib.check(_lib.load().b200_groth16_prove_batch(pk._handle, k, arrays["W"], arrays["A"], arrays["B"], arrays["C"],
+                                                    n_constraints, p(r), p(s), p(ar), p(bs), p(krs), p(msm)))
+    return [Proof(Ar=ar[i], Bs=bs[i], Krs=krs[i], msm=msm[i] if keep_msm else None) for i in range(k)]
+
+
+def ProveBatch(r1cs, pk: ProvingKey, full_witnesses, *opts: Option) -> List[Proof]:
+    """Prove for several witnesses of one circuit: each is solved, then all are proven in one ProveSolutionBatch call."""
+    return ProveSolutionBatch(pk, [r1cs.Solve(w) for w in full_witnesses], *opts)
+
+
 def Prove(r1cs, pk: ProvingKey, full_witness, *opts: Option) -> Proof:
     """groth16_icicle.go:79-98.  `r1cs.Solve(full_witness)` must return an R1CSSolution
     (the solver itself is CPU code outside this backend, as in the reference)."""

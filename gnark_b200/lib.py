@@ -39,7 +39,7 @@ EXPORTS = [
     "b200_comm_unique_id", "b200_comm_init", "b200_comm_init_all", "b200_comm_destroy", "b200_comm_info",
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
-    "b200_points_ntt", "b200_msm_indexed", "b200_msm_batch",
+    "b200_points_ntt", "b200_msm_indexed", "b200_msm_batch", "b200_ntt_batch", "b200_groth16_prove_batch",
 ]
 COMM_ID_BYTES = 128
 
@@ -186,6 +186,8 @@ def load(path: str = None):
     lib.b200_ntt_domain_free.argtypes = [vp]
     lib.b200_ntt.argtypes = [vp, vp, i32, i32, i32, i32]
     lib.b200_ntt_async.argtypes = [vp, vp, i32, i32, i32]
+    if "b200_ntt_batch" not in missing:
+        lib.b200_ntt_batch.argtypes = [vp, vp, sz, i32, i32, i32, i32]
     if "b200_points_ntt" not in missing:
         lib.b200_points_ntt.argtypes = [vp, i32, vp, i32, i32]
     lib.b200_groth16_compute_h.argtypes = [vp, vp, vp, vp, sz, i32, vp, i32]
@@ -207,6 +209,9 @@ def load(path: str = None):
     lib.b200_groth16_prove.argtypes = [vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp]
     lib.b200_groth16_msms.argtypes = [vp, vp, vp, vp, vp, sz, vp]
     lib.b200_groth16_assemble.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    if "b200_groth16_prove_batch" not in missing:
+        pp = ctypes.POINTER(vp)
+        lib.b200_groth16_prove_batch.argtypes = [vp, sz, pp, pp, pp, pp, sz, vp, vp, vp, vp, vp, vp]
     if path is None:
         _lib = lib
     return lib
@@ -488,6 +493,17 @@ class Domain:
     def ntt(self, data, inverse=False, decimation=DIF, on_coset=False, on_device=False):
         check(load().b200_ntt(self.handle, ptr(data), 1 if on_device else 0, 1 if inverse else 0, decimation,
                               1 if on_coset else 0))
+        return data
+
+    def ntt_batch(self, data, inverse=False, decimation=DIF, on_coset=False, on_device=False):
+        """In place on `batch` vectors of this domain's size in one call (item-major: batch * n * fr_limbs words, a
+        host array or a contiguous device tensor), each transformed as ntt() would."""
+        total = data.numel() if on_device else data.size
+        per = self.n * self.fr_limbs
+        if total % per:
+            raise ValueError(f"ntt_batch: {total} words is not a whole number of {self.n}-element vectors")
+        check(load().b200_ntt_batch(self.handle, ptr(data), total // per, 1 if on_device else 0, 1 if inverse else 0,
+                                    decimation, 1 if on_coset else 0))
         return data
 
     def ntt_async(self, d_data, inverse=False, decimation=DIF, on_coset=False):

@@ -146,82 +146,17 @@ func (pk *ProvingKey) setupDevicePointers(r1cs *cs.R1CS, cfg *b200.Config) error
 // option handling as the ICICLE backend's per-curve Prove (icicle.go:784); the stage order follows
 // backend/groth16/bn254/prove.go:52-315.
 func Prove(r1cs *cs.R1CS, pk *ProvingKey, fullWitness witness.Witness, cfg *b200.Config) (*groth16_bn254.Proof, error) {
-	opt, err := backend.NewProverConfig(cfg.ProverOpts...)
-	if err != nil {
-		return nil, fmt.Errorf("new prover config: %w", err)
-	}
-	if opt.HashToFieldFn == nil {
-		opt.HashToFieldFn = hash_to_field.New([]byte(constraint.CommitmentDst))
-	}
 	log := logger.Logger().With().Str("curve", r1cs.CurveID().String()).Str("acceleration", "b200").Int("nbConstraints", r1cs.GetNbConstraints()).Str("backend", "groth16").Logger()
 	if err := pk.setupDevicePointers(r1cs, cfg); err != nil {
 		return nil, fmt.Errorf("setup device pointers: %w", err)
 	}
 	info := pk.deviceInfo
-
-	commitmentInfo := r1cs.CommitmentInfo.(constraint.Groth16Commitments)
-	proof := &groth16_bn254.Proof{Commitments: make([]curve.G1Affine, len(commitmentInfo))}
-	solverOpts := opt.SolverOpts[:len(opt.SolverOpts):len(opt.SolverOpts)]
-	poks := make([]curve.G1Affine, len(pk.CommitmentKeys))
-
-	// override hints (prove.go:72-99): Commit AND ProveKnowledge of commitment i are two MSMs of the same scalars, run
-	// on the device over one upload; the proof of knowledge is kept for the fold below
-	bsb22ID := solver.GetHintID(fcs.Bsb22CommitmentComputePlaceholder)
-	solverOpts = append(solverOpts, solver.OverrideHint(bsb22ID, func(_ *big.Int, in []*big.Int, out []*big.Int) error {
-		i := int(in[0].Int64())
-		in = in[1:]
-		values := make([]fr.Element, len(commitmentInfo[i].PrivateCommitted))
-		hashed := in[:len(commitmentInfo[i].PublicAndCommitmentCommitted)]
-		committed := in[+len(hashed):]
-		for j, inJ := range committed {
-			values[j].SetBigInt(inJ)
-		}
-		var pinner runtime.Pinner
-		pinner.Pin(&proof.Commitments[i])
-		pinner.Pin(&poks[i])
-		if len(values) > 0 {
-			pinner.Pin(unsafe.SliceData(values))
-		}
-		err := info.commitment[i].Commit(ptrOf(values), len(values), unsafe.Pointer(&proof.Commitments[i]), unsafe.Pointer(&poks[i]))
-		pinner.Unpin()
-		if err != nil {
-			return err
-		}
-
-		opt.HashToFieldFn.Write(constraint.SerializeCommitment(proof.Commitments[i].Marshal(), hashed, (fr.Bits-1)/8+1))
-		hashBts := opt.HashToFieldFn.Sum(nil)
-		opt.HashToFieldFn.Reset()
-		nbBuf := fr.Bytes
-		if opt.HashToFieldFn.Size() < fr.Bytes {
-			nbBuf = opt.HashToFieldFn.Size()
-		}
-		var res fr.Element
-		res.SetBytes(hashBts[:nbBuf])
-		res.BigInt(out[0])
-		return nil
-	}))
-
-	_solution, err := r1cs.Solve(fullWitness, solverOpts...)
+	proof, solution, err := solve(r1cs, pk, fullWitness, cfg, info)
 	if err != nil {
 		return nil, err
 	}
-	solution := _solution.(*cs.R1CSSolution)
-	wireValues := []fr.Element(solution.W)
 
 	start := time.Now()
-
-	// compute challenge for folding the PoKs from the commitments (prove.go:118-129)
-	commitmentsSerialized := make([]byte, fr.Bytes*len(commitmentInfo))
-	for i := range commitmentInfo {
-		copy(commitmentsSerialized[fr.Bytes*i:], wireValues[commitmentInfo[i].CommitmentIndex].Marshal())
-	}
-	challenge, err := fr.Hash(commitmentsSerialized, []byte("G16-BSB22"), 1)
-	if err != nil {
-		return nil, err
-	}
-	if _, err = proof.CommitmentPok.Fold(poks, challenge[0], ecc.MultiExpConfig{NbTasks: 1}); err != nil {
-		return nil, err
-	}
 
 	// sample random r and s (prove.go:170-182)
 	var r, s fr.Element
@@ -284,4 +219,146 @@ func Prove(r1cs *cs.R1CS, pk *ProvingKey, fullWitness witness.Witness, cfg *b200
 	runtime.KeepAlive(solution)
 	log.Debug().Dur("took", time.Since(start)).Msg("prover done")
 	return proof, nil
+}
+
+// solve runs the R1CS solver with the BSB22 commitment hint served by the device (prove.go:72-99) and folds the proofs of
+// knowledge of the commitments (prove.go:118-129).  Every call has its own prover config, hint closure and proof, so
+// several witnesses can be solved concurrently.
+func solve(r1cs *cs.R1CS, pk *ProvingKey, fullWitness witness.Witness, cfg *b200.Config, info *deviceInfo) (*groth16_bn254.Proof, *cs.R1CSSolution, error) {
+	opt, err := backend.NewProverConfig(cfg.ProverOpts...)
+	if err != nil {
+		return nil, nil, fmt.Errorf("new prover config: %w", err)
+	}
+	if opt.HashToFieldFn == nil {
+		opt.HashToFieldFn = hash_to_field.New([]byte(constraint.CommitmentDst))
+	}
+	commitmentInfo := r1cs.CommitmentInfo.(constraint.Groth16Commitments)
+	proof := &groth16_bn254.Proof{Commitments: make([]curve.G1Affine, len(commitmentInfo))}
+	solverOpts := opt.SolverOpts[:len(opt.SolverOpts):len(opt.SolverOpts)]
+	poks := make([]curve.G1Affine, len(pk.CommitmentKeys))
+	// override hints (prove.go:72-99): Commit AND ProveKnowledge of commitment i are two MSMs of the same scalars, run
+	// on the device over one upload; the proof of knowledge is kept for the fold below
+	bsb22ID := solver.GetHintID(fcs.Bsb22CommitmentComputePlaceholder)
+	solverOpts = append(solverOpts, solver.OverrideHint(bsb22ID, func(_ *big.Int, in []*big.Int, out []*big.Int) error {
+		i := int(in[0].Int64())
+		in = in[1:]
+		values := make([]fr.Element, len(commitmentInfo[i].PrivateCommitted))
+		hashed := in[:len(commitmentInfo[i].PublicAndCommitmentCommitted)]
+		committed := in[+len(hashed):]
+		for j, inJ := range committed {
+			values[j].SetBigInt(inJ)
+		}
+		var pinner runtime.Pinner
+		pinner.Pin(&proof.Commitments[i])
+		pinner.Pin(&poks[i])
+		if len(values) > 0 {
+			pinner.Pin(unsafe.SliceData(values))
+		}
+		err := info.commitment[i].Commit(ptrOf(values), len(values), unsafe.Pointer(&proof.Commitments[i]), unsafe.Pointer(&poks[i]))
+		pinner.Unpin()
+		if err != nil {
+			return err
+		}
+
+		opt.HashToFieldFn.Write(constraint.SerializeCommitment(proof.Commitments[i].Marshal(), hashed, (fr.Bits-1)/8+1))
+		hashBts := opt.HashToFieldFn.Sum(nil)
+		opt.HashToFieldFn.Reset()
+		nbBuf := fr.Bytes
+		if opt.HashToFieldFn.Size() < fr.Bytes {
+			nbBuf = opt.HashToFieldFn.Size()
+		}
+		var res fr.Element
+		res.SetBytes(hashBts[:nbBuf])
+		res.BigInt(out[0])
+		return nil
+	}))
+
+	_solution, err := r1cs.Solve(fullWitness, solverOpts...)
+	if err != nil {
+		return nil, nil, err
+	}
+	solution := _solution.(*cs.R1CSSolution)
+	wireValues := []fr.Element(solution.W)
+
+	// compute challenge for folding the PoKs from the commitments (prove.go:118-129)
+	commitmentsSerialized := make([]byte, fr.Bytes*len(commitmentInfo))
+	for i := range commitmentInfo {
+		copy(commitmentsSerialized[fr.Bytes*i:], wireValues[commitmentInfo[i].CommitmentIndex].Marshal())
+	}
+	challenge, err := fr.Hash(commitmentsSerialized, []byte("G16-BSB22"), 1)
+	if err != nil {
+		return nil, nil, err
+	}
+	if _, err = proof.CommitmentPok.Fold(poks, challenge[0], ecc.MultiExpConfig{NbTasks: 1}); err != nil {
+		return nil, nil, err
+	}
+	return proof, solution, nil
+}
+
+
+// ProveBatch proves several full witnesses of one circuit with one b200_groth16_prove_batch call: the witnesses are solved
+// concurrently (each with its own hint closure, proof and proof-of-knowledge fold), then the device work of all of them
+// runs as one launch sequence.  Proof i equals what Prove gives for witness i with the same r, s.  One device and an
+// unsharded key only.
+func ProveBatch(r1cs *cs.R1CS, pk *ProvingKey, fullWitnesses []witness.Witness, cfg *b200.Config) ([]*groth16_bn254.Proof, error) {
+	if len(cfg.Devices()) > 1 {
+		return nil, fmt.Errorf("ProveBatch: one device only (WithDevices lists %d)", len(cfg.Devices()))
+	}
+	if len(fullWitnesses) == 0 {
+		return nil, nil
+	}
+	if err := pk.setupDevicePointers(r1cs, cfg); err != nil {
+		return nil, fmt.Errorf("setup device pointers: %w", err)
+	}
+	info := pk.deviceInfo
+	k := len(fullWitnesses)
+	proofs := make([]*groth16_bn254.Proof, k)
+	solutions := make([]*cs.R1CSSolution, k)
+	errs := make([]error, k)
+	var wg sync.WaitGroup
+	for i := range fullWitnesses {
+		wg.Add(1)
+		go func(i int) {
+			defer wg.Done()
+			proofs[i], solutions[i], errs[i] = solve(r1cs, pk, fullWitnesses[i], cfg, info)
+		}(i)
+	}
+	wg.Wait()
+	for i, e := range errs {
+		if e != nil {
+			return nil, fmt.Errorf("witness %d: %w", i, e)
+		}
+	}
+	// r_i, s_i item-major (prove.go:170-182); the outputs are written into the proofs through three staging arrays
+	rs := make([]fr.Element, 2*k)
+	for i := range rs {
+		if _, err := rs[i].SetRandom(); err != nil {
+			return nil, err
+		}
+	}
+	r, s := make([]fr.Element, k), make([]fr.Element, k)
+	for i := 0; i < k; i++ {
+		r[i], s[i] = rs[2*i], rs[2*i+1]
+	}
+	ar, bs, krs := make([]curve.G1Affine, k), make([]curve.G2Affine, k), make([]curve.G1Affine, k)
+	var pinner runtime.Pinner
+	defer pinner.Unpin()
+	w, a, b, c := make([]unsafe.Pointer, k), make([]unsafe.Pointer, k), make([]unsafe.Pointer, k), make([]unsafe.Pointer, k)
+	for i, sol := range solutions {
+		for _, p := range []any{unsafe.SliceData(sol.W), unsafe.SliceData(sol.A), unsafe.SliceData(sol.B), unsafe.SliceData(sol.C)} {
+			pinner.Pin(p)
+		}
+		w[i], a[i], b[i], c[i] = ptrOf(sol.W), ptrOf(sol.A), ptrOf(sol.B), ptrOf(sol.C)
+	}
+	for _, p := range []any{unsafe.SliceData(r), unsafe.SliceData(s), unsafe.SliceData(ar), unsafe.SliceData(bs), unsafe.SliceData(krs)} {
+		pinner.Pin(p)
+	}
+	if err := info.keys[0].ProveBatch(w, a, b, c, len(solutions[0].A), ptrOf(r), ptrOf(s), ptrOf(ar), ptrOf(bs), ptrOf(krs)); err != nil {
+		return nil, err
+	}
+	for i := range proofs {
+		proofs[i].Ar, proofs[i].Bs, proofs[i].Krs = ar[i], bs[i], krs[i]
+	}
+	runtime.KeepAlive(solutions)
+	return proofs, nil
 }

@@ -54,6 +54,51 @@ func Prove(r1cs constraint.ConstraintSystem, pk groth16.ProvingKey, fullWitness 
 	}
 }
 
+// ProveBatch generates one proof per full witness of one r1cs in a single device call: the witnesses are solved
+// concurrently, then every proof's device work runs as one batch (batched NTTs and one batched MSM per key table), which
+// pays the fixed cost of the MSM and NTT pipelines once for all of them.  Proof i is what Prove would give for witness i
+// with the same randomness.  One device only: WithDevices with more than one device is an error.
+//
+// NB! the provided proving key must be a B200 proving key.
+func ProveBatch(r1cs constraint.ConstraintSystem, pk groth16.ProvingKey, fullWitnesses []witness.Witness, opts ...b200.Option) ([]groth16.Proof, error) {
+	config, err := b200.NewConfig(opts...)
+	if err != nil {
+		return nil, fmt.Errorf("initializing config: %w", err)
+	}
+	if err := cabi.Init(config.Devices()); err != nil {
+		panic(fmt.Sprintf("b200 device initialisation: %v", err))
+	}
+	out := make([]groth16.Proof, len(fullWitnesses))
+	switch _r1cs := r1cs.(type) {
+	case *cs_bls12377.R1CS:
+		proofs, err := b200_bls12377.ProveBatch(_r1cs, pk.(*b200_bls12377.ProvingKey), fullWitnesses, config)
+		for i, p := range proofs {
+			out[i] = p
+		}
+		return out, err
+	case *cs_bls12381.R1CS:
+		proofs, err := b200_bls12381.ProveBatch(_r1cs, pk.(*b200_bls12381.ProvingKey), fullWitnesses, config)
+		for i, p := range proofs {
+			out[i] = p
+		}
+		return out, err
+	case *cs_bn254.R1CS:
+		proofs, err := b200_bn254.ProveBatch(_r1cs, pk.(*b200_bn254.ProvingKey), fullWitnesses, config)
+		for i, p := range proofs {
+			out[i] = p
+		}
+		return out, err
+	case *cs_bw6761.R1CS:
+		proofs, err := b200_bw6761.ProveBatch(_r1cs, pk.(*b200_bw6761.ProvingKey), fullWitnesses, config)
+		for i, p := range proofs {
+			out[i] = p
+		}
+		return out, err
+	default:
+		panic("b200 backend requested but r1cs is not of a supported curve")
+	}
+}
+
 // Setup generates a proving and verifying key for a given r1cs.
 //
 // The method wraps the [groth16.Setup] method, but the returned proving key is a B200 proving key. To convert the key

@@ -18,6 +18,13 @@ func Prove(r1cs constraint.ConstraintSystem, pk groth16.ProvingKey, fullWitness 
 	panic("b200 backend requested but program compiled without 'b200' build tag")
 }
 
+// ProveBatch generates one proof per full witness of one r1cs in a single device call.
+//
+// NB! the provided proving key must be a B200 proving key.
+func ProveBatch(r1cs constraint.ConstraintSystem, pk groth16.ProvingKey, fullWitnesses []witness.Witness, opts ...b200.Option) ([]groth16.Proof, error) {
+	panic("b200 backend requested but program compiled without 'b200' build tag")
+}
+
 // Setup generates a proving and verifying key for a given r1cs.
 //
 // The method wraps the [groth16.Setup] method, but the returned proving key is a B200 proving key. To convert the key

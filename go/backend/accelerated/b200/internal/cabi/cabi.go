@@ -147,6 +147,29 @@ func (k *Groth16Key) Prove(w, a, b, c unsafe.Pointer, nConstraints int, r, s, ar
 	})
 }
 
+// ProveBatch is b200_groth16_prove_batch: len(w) proofs of one circuit in one call.  w, a, b, c: one pointer per item to
+// the first element of its fr.Vectors (the C arrays of pointers are built here, as Begin does for pi2); r, s: len(w)
+// fr.Elements each; ar, bs, krs: len(w) proof points each.
+func (k *Groth16Key) ProveBatch(w, a, b, c []unsafe.Pointer, nConstraints int, r, s, ar, bs, krs unsafe.Pointer) error {
+	n := len(w)
+	if n == 0 {
+		return nil
+	}
+	if len(a) != n || len(b) != n || len(c) != n {
+		return errors.New("ProveBatch: w, a, b, c must have one pointer per item")
+	}
+	arrays := [4]*unsafe.Pointer{}
+	for i, src := range [4][]unsafe.Pointer{w, a, b, c} {
+		arrays[i] = (*unsafe.Pointer)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(uintptr(0)))))
+		defer C.free(unsafe.Pointer(arrays[i]))
+		copy(unsafe.Slice(arrays[i], n), src)
+	}
+	return Call(func() int32 {
+		return int32(C.b200_groth16_prove_batch(k.h, C.size_t(n), arrays[0], arrays[1], arrays[2], arrays[3],
+			C.size_t(nConstraints), r, s, ar, bs, krs, nil))
+	})
+}
+
 // MSMs is b200_groth16_msms: this shard's partial sums, 4 G1Jac + 1 G2Jac into out.
 func (k *Groth16Key) MSMs(w, a, b, c unsafe.Pointer, nConstraints int, out unsafe.Pointer) error {
 	return Call(func() int32 { return int32(C.b200_groth16_msms(k.h, w, a, b, c, C.size_t(nConstraints), out)) })

@@ -239,6 +239,10 @@ int32_t b200_ntt_domain_free(b200_domain_t d);
 int32_t b200_ntt(b200_domain_t d, void* data, int32_t data_on_dev, int32_t inverse, int32_t decimation,
                  int32_t on_coset);
 int32_t b200_ntt_async(b200_domain_t d, void* d_data, int32_t inverse, int32_t decimation, int32_t on_coset);
+/* `batch` transforms of the domain's size in one call (ICICLE's NTTConfig.BatchSize): data holds batch * 2^log2n
+ * fr.Elements item-major, each vector transformed as b200_ntt would.  batch = 0 does nothing. */
+int32_t b200_ntt_batch(b200_domain_t d, void* data, size_t batch, int32_t data_on_dev, int32_t inverse,
+                       int32_t decimation, int32_t on_coset);
 /* Group-element NTT: a KZG SRS between monomial form [tau^k]G and the Lagrange basis [L_i(tau)]G (SURVEY.md §8(f)-3).
  * Replaces gnark-crypto's kzg.ToLagrangeG1 (as used at std/recursion/plonk/verifier_test.go:370; in-tree statement
  * lagrangeCoeffsG1, backend/groth16/<curve>/mpcsetup/lagrange.go:21-41), the route of a ceremony SRS without a trapdoor;
@@ -463,6 +467,17 @@ int32_t b200_groth16_msms(b200_pk_t pk, const void* wires, const void* a, const 
                           size_t n_constraints, void* msm_out);
 int32_t b200_groth16_assemble(b200_pk_t pk, const void* msm5, const void* r, const void* s, void* ar_out,
                               void* bs_out, void* krs_out);
+/* `batch` proofs of one circuit in one call: the device work of all items runs as one launch sequence (batched
+ * wire filters, one batched MSM per key table, computeH as batched NTTs), then the proofs are assembled on host threads.
+ * wires / a / b / c: one host pointer per item (nb_wires and n_constraints fr.Elements, as b200_groth16_prove takes);
+ * r, s: batch fr.Elements each, item-major.  Outputs: batch affine points each in ar_out, bs_out, krs_out; msm_out
+ * (optional) batch x (4 G1Jac + 1 G2Jac), each item laid out as b200_groth16_prove's.  Every proof equals what
+ * b200_groth16_prove gives for the same item and r, s.  Refused, with every output untouched: sharded keys, a null
+ * argument, n_constraints above the domain, and a batch larger than the device indices allow (the message names the
+ * largest batch the key takes).  batch = 0 writes nothing. */
+int32_t b200_groth16_prove_batch(b200_pk_t pk, size_t batch, const void* const* wires, const void* const* a,
+                                 const void* const* b, const void* const* c, size_t n_constraints,
+                                 const void* r, const void* s, void* ar_out, void* bs_out, void* krs_out, void* msm_out);
 
 #ifdef __cplusplus
 }
