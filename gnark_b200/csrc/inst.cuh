@@ -1,6 +1,8 @@
 // Per-curve instantiation of the kernel templates behind the type-erased tables of
 // internal.h.  Included by inst_<curve>.cu only.
 #pragma once
+#include <vector>
+
 #include "host_field.h"
 #include "internal.h"
 #include "fixed_base.cuh"
@@ -378,6 +380,69 @@ struct NttInst {
     GB_CUDA_TRY(pwb.release_on(st)); GB_CUDA_TRY(pwib.release_on(st));
     return cudaStreamSynchronize(st);
   }
+  // ---- batches of polynomials (item-major rows of n coefficients), enqueued on `st` without a host synchronisation:
+  // the point tables go up in one copy from a pageable host buffer, which cudaMemcpyAsync has consumed when it returns
+  static cudaError_t upload_pow_tables(cudaStream_t st, const Fr* pts, size_t batch, uint32_t len, bool with_inv,
+                                       AsyncBuf& d_pw) {
+    std::vector<Fr> tab((with_inv ? 2 : 1) * batch * len);
+    kzg_pow_tables<Fr>(pts, batch, len, with_inv, tab.data());
+    GB_CUDA_TRY(d_pw.alloc(tab.size() * sizeof(Fr), st));
+    return cudaMemcpyAsync(d_pw.p, tab.data(), tab.size() * sizeof(Fr), cudaMemcpyHostToDevice, st);
+  }
+  // d_values[b] = p_b(points[b]); points on the host
+  static cudaError_t poly_eval_batch(cudaStream_t st, const void* polys, size_t n, size_t batch, const void* points_host,
+                                     void* d_values) {
+    if (!batch) return cudaSuccess;
+    if (n == 0) return cudaMemsetAsync(d_values, 0, batch * sizeof(Fr), st);
+    const uint32_t len = kzg_pow_len(n);
+    AsyncBuf pwb, sumsb;
+    GB_CUDA_TRY(upload_pow_tables(st, (const Fr*)points_host, batch, len, false, pwb));
+    const size_t nblocks = (n + 256 * EVAL_E - 1) / (256 * EVAL_E);
+    GB_CUDA_TRY(sumsb.alloc(batch * nblocks * sizeof(Fr), st));
+    const Fr *c = (const Fr*)polys, *pw = (const Fr*)pwb.p;
+    Fr *sums = (Fr*)sumsb.p, *vals = (Fr*)d_values;
+    for (size_t b0 = 0; b0 < batch; b0 += NTT_MAX_GRID_Y) {
+      const unsigned rows = (unsigned)(batch - b0 < NTT_MAX_GRID_Y ? batch - b0 : NTT_MAX_GRID_Y);
+      k_poly_eval_partial<Fr, true><<<dim3((unsigned)nblocks, rows), 256, 0, st>>>(c + b0 * n, n, pw + b0 * len, Fr::zero(),
+                                                                                 sums + b0 * nblocks, len);
+      k_sum_reduce<Fr, true><<<dim3(1, rows), 256, 0, st>>>(sums + b0 * nblocks, nblocks, vals + b0);
+      GB_CUDA_TRY(cudaGetLastError());
+    }
+    GB_CUDA_TRY(sumsb.release_on(st));
+    return pwb.release_on(st);
+  }
+  // row b of d_q <- (p_b(X) - p_b(z_b)) / (X - z_b) (top coefficient zeroed), d_values[b] <- p_b(z_b); the polynomials
+  // are only read.  Points on the host; a point of 0 divides by X.
+  static cudaError_t poly_div_linear_batch(cudaStream_t st, const void* polys, size_t n, size_t batch,
+                                           const void* points_host, void* d_q, void* d_values) {
+    if (!batch) return cudaSuccess;
+    if (n == 0) return cudaMemsetAsync(d_values, 0, batch * sizeof(Fr), st);
+    const uint32_t len = kzg_pow_len(n);
+    AsyncBuf pwb, tb;
+    GB_CUDA_TRY(upload_pow_tables(st, (const Fr*)points_host, batch, len, true, pwb));
+    GB_CUDA_TRY(tb.alloc(batch * n * sizeof(Fr), st));
+    const Fr *c = (const Fr*)polys, *pw = (const Fr*)pwb.p, *pwi = pw + batch * len;
+    Fr *t = (Fr*)tb.p, *q = (Fr*)d_q, *vals = (Fr*)d_values;
+    const unsigned nb = (unsigned)((n + 256 * EVAL_E - 1) / (256 * EVAL_E));
+    for (size_t b0 = 0; b0 < batch; b0 += NTT_MAX_GRID_Y) {
+      const unsigned rows = (unsigned)(batch - b0 < NTT_MAX_GRID_Y ? batch - b0 : NTT_MAX_GRID_Y);
+      const size_t off = b0 * n;
+      k_syndiv_pre<Fr, true><<<dim3(nb, rows), 256, 0, st>>>(c + off, n, pwi + b0 * len, Fr::zero(), t + off, len);
+      GB_CUDA_TRY(cudaGetLastError());
+      GB_CUDA_TRY((scan_enqueue<Fr, 1, true>(st, t + off, n, false, rows)));
+      k_syndiv_post<Fr, true><<<dim3(nb, rows), 256, 0, st>>>(t + off, n, pw + b0 * len, Fr::zero(), q + off, vals + b0, len,
+                                                             c + off);
+      GB_CUDA_TRY(cudaGetLastError());
+    }
+    GB_CUDA_TRY(tb.release_on(st));
+    return pwb.release_on(st);
+  }
+  // d_out[j] = sum_b gamma^b p_b[j], j < n (batch >= 1)
+  static cudaError_t poly_fold(cudaStream_t st, const void* polys, size_t n, size_t batch, const void* gamma, void* d_out) {
+    if (!n || !batch) return cudaSuccess;
+    k_poly_fold<Fr><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const Fr*)polys, n, batch, *(const Fr*)gamma, (Fr*)d_out);
+    return cudaGetLastError();
+  }
   static cudaError_t gather(cudaStream_t st, void* out, const void* src, const uint32_t* idx, size_t n) {
     if (!n) return cudaSuccess;
     k_gather<Fr><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((Fr*)out, (const Fr*)src, idx, n);
@@ -403,7 +468,8 @@ struct NttInst {
     static const NttOps o = {sizeof(Fr), Fr::Params::TWO_ADICITY, &domain_new, &domain_free, &domain_bytes, &ntt,
                              &compute_h, &vec_op, &bit_reverse, &scale_powers, &batch_invert, &plonk_coset,
                              &plonk_divide_by_zh, &axpy, &scan, &plonk_build_z, &poly_eval, &poly_div_linear, &gather,
-                             &host_fr, &plonk_bsb22, &ntt_batch, &compute_h_batch, &gather_batch};
+                             &host_fr, &plonk_bsb22, &ntt_batch, &compute_h_batch, &gather_batch,
+                             &poly_eval_batch, &poly_div_linear_batch, &poly_fold};
     return &o;
   }
 };

@@ -110,6 +110,15 @@ struct NttOps {
   // gather over a batch: out[b * out_stride + j] = src[b * src_stride + idx[j]], j < n, b < batch
   cudaError_t (*gather_batch)(cudaStream_t st, void* d_out, const void* d_src, const uint32_t* d_idx, size_t n, size_t batch,
                               size_t src_stride, size_t out_stride);
+  // batches of `batch` polynomials of n coefficients, item-major on the device, points on the host; enqueued on st with
+  // no host synchronisation (plonk.cuh): d_values[b] = p_b(points[b]) ...
+  cudaError_t (*poly_eval_batch)(cudaStream_t st, const void* d_polys, size_t n, size_t batch, const void* points_host,
+                                 void* d_values);
+  // ... row b of d_q (batch * n) = (p_b - p_b(z_b)) / (X - z_b) with its top coefficient 0, d_values[b] = p_b(z_b) ...
+  cudaError_t (*poly_div_linear_batch)(cudaStream_t st, const void* d_polys, size_t n, size_t batch, const void* points_host,
+                                       void* d_q, void* d_values);
+  // ... d_out[j] = sum_b gamma^b p_b[j] (n coefficients; gamma on the host)
+  cudaError_t (*poly_fold)(cudaStream_t st, const void* d_polys, size_t n, size_t batch, const void* gamma_mont, void* d_out);
 };
 
 // Host-side group arithmetic for proof assembly (backend/groth16/bn254/prove.go:

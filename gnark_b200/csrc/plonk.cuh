@@ -183,12 +183,27 @@ HD Fr scan_op(const Fr& a, const Fr& b) { return OP == 0 ? a * b : a + b; }
 template <class Fr, int OP>
 HD Fr scan_identity() { return OP == 0 ? Fr::one() : Fr::zero(); }
 
+// x^k by square-and-multiply from pw[j] = x^(2^j)
+template <class Fr>
+HD Fr pow_from_table(const Fr* __restrict__ pw, size_t k) {
+  Fr acc = Fr::one();
+  for (int j = 0; k; j++, k >>= 1)
+    if (k & 1) acc = acc * pw[j];
+  return acc;
+}
+
 #ifdef __CUDACC__
-// block-local scan of SCAN_THREADS*SCAN_E elements; block totals to block_sums (nullable)
-template <class Fr, int OP>
+// block-local scan of SCAN_THREADS*SCAN_E elements; block totals to block_sums (nullable).  kBatch: blockIdx.y selects
+// the row (n elements at data + row * n) and the row's block totals go to block_sums + row * gridDim.x; blocks never
+// span two rows.
+template <class Fr, int OP, bool kBatch = false>
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_block(Fr* __restrict__ data, size_t n, Fr* __restrict__ block_sums,
                                                              int exclusive) {
   __shared__ Fr sm[SCAN_THREADS];
+  if (kBatch) {
+    data += (size_t)blockIdx.y * n;
+    if (block_sums) block_sums += (size_t)blockIdx.y * gridDim.x;
+  }
   const size_t base = ((size_t)blockIdx.x * SCAN_THREADS + threadIdx.x) * SCAN_E;
   Fr v[SCAN_E];
 #pragma unroll
@@ -213,10 +228,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_block(Fr* __restrict__ da
     else data[base + k] = scan_op<Fr, OP>(prefix, v[k]);
   }
 }
-template <class Fr, int OP>
+template <class Fr, int OP, bool kBatch = false>
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_fix(Fr* __restrict__ data, size_t n,
                                                            const Fr* __restrict__ block_prefix) {
   if (blockIdx.x == 0) return;
+  if (kBatch) {
+    data += (size_t)blockIdx.y * n;
+    block_prefix += (size_t)blockIdx.y * gridDim.x;
+  }
   const Fr p = block_prefix[blockIdx.x];
   const size_t base = ((size_t)blockIdx.x * SCAN_THREADS + threadIdx.x) * SCAN_E;
 #pragma unroll
@@ -224,36 +243,28 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_fix(Fr* __restrict__ data
     if (base + k < n) data[base + k] = scan_op<Fr, OP>(p, data[base + k]);
 }
 
-// in-place scan of n elements on `st` (recursive over block totals)
-template <class Fr, int OP>
-cudaError_t scan_enqueue(cudaStream_t st, Fr* data, size_t n, bool exclusive) {
+// in-place scan of n elements on `st` (recursive over block totals).  kBatch: `rows` (<= 65 535, the grid's y limit)
+// independent scans of n elements each, item-major, their block totals scanned per row.
+template <class Fr, int OP, bool kBatch = false>
+cudaError_t scan_enqueue(cudaStream_t st, Fr* data, size_t n, bool exclusive, unsigned rows = 1) {
   if (n == 0) return cudaSuccess;
   const size_t per_block = (size_t)SCAN_THREADS * SCAN_E;
   const size_t nblocks = (n + per_block - 1) / per_block;
   if (nblocks == 1) {
-    k_scan_block<Fr, OP><<<1, SCAN_THREADS, 0, st>>>(data, n, nullptr, exclusive ? 1 : 0);
+    k_scan_block<Fr, OP, kBatch><<<dim3(1, rows), SCAN_THREADS, 0, st>>>(data, n, nullptr, exclusive ? 1 : 0);
     return cudaGetLastError();
   }
   Fr* sums = nullptr;
-  cudaError_t e = cudaMallocAsync(&sums, nblocks * sizeof(Fr), st);
+  cudaError_t e = cudaMallocAsync(&sums, (size_t)rows * nblocks * sizeof(Fr), st);
   if (e != cudaSuccess) return e;
-  k_scan_block<Fr, OP><<<(unsigned)nblocks, SCAN_THREADS, 0, st>>>(data, n, sums, exclusive ? 1 : 0);
-  e = scan_enqueue<Fr, OP>(st, sums, nblocks, true);
+  k_scan_block<Fr, OP, kBatch><<<dim3((unsigned)nblocks, rows), SCAN_THREADS, 0, st>>>(data, n, sums, exclusive ? 1 : 0);
+  e = scan_enqueue<Fr, OP, kBatch>(st, sums, nblocks, true, rows);
   if (e == cudaSuccess) {
-    k_scan_fix<Fr, OP><<<(unsigned)nblocks, SCAN_THREADS, 0, st>>>(data, n, sums);
+    k_scan_fix<Fr, OP, kBatch><<<dim3((unsigned)nblocks, rows), SCAN_THREADS, 0, st>>>(data, n, sums);
     e = cudaGetLastError();
   }
   cudaError_t e2 = cudaFreeAsync(sums, st);
   return e != cudaSuccess ? e : e2;
-}
-
-// x^k by square-and-multiply from pw[j] = x^(2^j)
-template <class Fr>
-DEV Fr pow_from_table(const Fr* __restrict__ pw, size_t k) {
-  Fr acc = Fr::one();
-  for (int j = 0; k; j++, k >>= 1)
-    if (k & 1) acc = acc * pw[j];
-  return acc;
 }
 
 // permutation ratios: num[i] = prod_j (f_j[i] + beta*id_j(i) + gamma), den[i] = prod_j (f_j[i] + beta*supp[S[j n+i]] + gamma)
@@ -294,47 +305,29 @@ __global__ void __launch_bounds__(256) k_plonk_shift_ratio(uint32_t n, const Fr*
   z[i] = i == 0 ? Fr::one() : num[i - 1] * den_inv[i - 1];
 }
 
-// polynomial evaluation: block partial sums of c_i x^i
+#endif
+
+// ---- per-thread steps of evaluation and division (shared by the kernels below and their host emulation) ----
+// Thread t of block blk handles the EVAL_E coefficients from base = (blk * 256 + t) * EVAL_E of its polynomial.
 constexpr int EVAL_E = 8;
+
+// the thread's share of p(x): sum_{k < EVAL_E} c[base + k] x^(base + k)  (zero past the end)
 template <class Fr>
-__global__ void __launch_bounds__(256) k_poly_eval_partial(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw,
-                                                           Fr x, Fr* __restrict__ block_sums) {
-  __shared__ Fr sm[256];
-  const size_t base = ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E;
+HD Fr poly_eval_chunk(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw, const Fr& x, size_t base) {
   Fr acc = Fr::zero();
   if (base < n) {
 #pragma unroll
     for (int k = EVAL_E - 1; k >= 0; k--) acc = acc * x + (base + k < n ? c[base + k] : Fr::zero());
     acc = acc * pow_from_table<Fr>(pw, base);
   }
-  sm[threadIdx.x] = acc;
-  __syncthreads();
-  for (int w = 128; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) sm[threadIdx.x] = sm[threadIdx.x] + sm[threadIdx.x + w];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) block_sums[blockIdx.x] = sm[0];
-}
-template <class Fr>
-__global__ void __launch_bounds__(256) k_sum_reduce(const Fr* __restrict__ v, size_t n, Fr* __restrict__ out) {
-  __shared__ Fr sm[256];
-  Fr acc = Fr::zero();
-  for (size_t i = threadIdx.x; i < n; i += 256) acc = acc + v[i];
-  sm[threadIdx.x] = acc;
-  __syncthreads();
-  for (int w = 128; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) sm[threadIdx.x] = sm[threadIdx.x] + sm[threadIdx.x + w];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *out = sm[0];
+  return acc;
 }
 
 // synthetic division by (X - z), z != 0:  t_k = c_{n-1-k} z^-k ; s = inclusive sum scan(t) ;
 // q_{n-2-k} = s_k z^k (k <= n-2) ; remainder = s_{n-1} z^(n-1) = p(z)
 template <class Fr>
-__global__ void __launch_bounds__(256) k_syndiv_pre(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw_inv,
-                                                    Fr zinv, Fr* __restrict__ t) {
-  const size_t base = ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E;
+HD void syndiv_pre_chunk(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw_inv, const Fr& zinv,
+                         Fr* __restrict__ t, size_t base) {
   if (base >= n) return;
   Fr p = pow_from_table<Fr>(pw_inv, base);
 #pragma unroll
@@ -345,9 +338,8 @@ __global__ void __launch_bounds__(256) k_syndiv_pre(const Fr* __restrict__ c, si
   }
 }
 template <class Fr>
-__global__ void __launch_bounds__(256) k_syndiv_post(const Fr* __restrict__ s, size_t n, const Fr* __restrict__ pw, Fr z,
-                                                     Fr* __restrict__ q, Fr* __restrict__ rem) {
-  const size_t base = ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E;
+HD void syndiv_post_chunk(const Fr* __restrict__ s, size_t n, const Fr* __restrict__ pw, const Fr& z, Fr* __restrict__ q,
+                          Fr* __restrict__ rem, size_t base) {
   if (base >= n) return;
   Fr p = pow_from_table<Fr>(pw, base);
 #pragma unroll
@@ -359,6 +351,140 @@ __global__ void __launch_bounds__(256) k_syndiv_post(const Fr* __restrict__ s, s
     else q[n - 2 - kk] = v;
     p = p * z;
   }
+}
+// division by X: q_i = c_{i+1}, q_{n-1} = 0, remainder c_0 (a batch item whose point is 0)
+template <class Fr>
+HD void syndiv_zero_chunk(const Fr* __restrict__ c, size_t n, Fr* __restrict__ q, Fr* __restrict__ rem, size_t base) {
+  for (int k = 0; k < EVAL_E; k++) {
+    const size_t kk = base + k;
+    if (kk >= n) break;
+    q[kk] = kk + 1 < n ? c[kk + 1] : Fr::zero();
+    if (kk == 0) *rem = c[0];
+  }
+}
+// out[j] = sum_b gamma^b p_b[j] over `batch` item-major polynomials of n coefficients (Horner in gamma, gamma^0 = 1)
+template <class Fr>
+HD Fr poly_fold_coeff(const Fr* __restrict__ polys, size_t n, size_t batch, const Fr& gamma, size_t j) {
+  Fr acc = polys[(batch - 1) * n + j];
+  for (size_t b = batch - 1; b-- > 0;) acc = acc * gamma + polys[b * n + j];
+  return acc;
+}
+
+// Power tables of a batch of points: entries j <= ceil(log2 n) of x^(2^j), which is every entry pow_from_table reads for
+// an exponent below n (and entry 0 is the point itself)
+HD uint32_t kzg_pow_len(size_t n) {
+  uint32_t l = 0;
+  while (l < 63 && ((size_t)1 << l) < n) l++;
+  return l + 1;
+}
+// out[b * len + j] = x_b^(2^j); with_inv: then out[(batch + b) * len + j] = x_b^(-2^j), the batch's inverses from ONE
+// inversion (Montgomery's trick; a zero point gets a zero table)
+template <class Fr>
+void kzg_pow_tables(const Fr* pts, size_t batch, uint32_t len, bool with_inv, Fr* out) {
+  for (int half = 0; half < (with_inv ? 2 : 1); half++) {
+    Fr* o = out + (size_t)half * batch * len;
+    if (half == 1) {
+      // prefix products of the non-zero points, one inversion, then back to front
+      Fr acc = Fr::one();
+      for (size_t b = 0; b < batch; b++) {
+        o[b * len] = acc;
+        if (!pts[b].is_zero()) acc = acc * pts[b];
+      }
+      Fr inv = acc.inverse();
+      for (size_t b = batch; b-- > 0;) {
+        if (pts[b].is_zero()) { o[b * len] = Fr::zero(); continue; }
+        o[b * len] = inv * o[b * len];
+        inv = inv * pts[b];
+      }
+    } else {
+      for (size_t b = 0; b < batch; b++) o[b * len] = pts[b];
+    }
+    for (size_t b = 0; b < batch; b++)
+      for (uint32_t j = 1; j < len; j++) o[b * len + j] = o[b * len + j - 1].sqr();
+  }
+}
+
+#ifdef __CUDACC__
+// polynomial evaluation: block partial sums of c_i x^i.  kBatch: blockIdx.y selects the polynomial (n coefficients at
+// c + row * n), whose point is pw[row * pw_len] (its table's entry 0) and whose block sums go to row `row` of
+// block_sums (gridDim.x each)
+template <class Fr, bool kBatch = false>
+__global__ void __launch_bounds__(256) k_poly_eval_partial(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw,
+                                                           Fr x, Fr* __restrict__ block_sums, uint32_t pw_len = 0) {
+  __shared__ Fr sm[256];
+  if (kBatch) {
+    c += (size_t)blockIdx.y * n;
+    pw += (size_t)blockIdx.y * pw_len;
+    x = pw[0];
+    block_sums += (size_t)blockIdx.y * gridDim.x;
+  }
+  const size_t base = ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E;
+  sm[threadIdx.x] = poly_eval_chunk<Fr>(c, n, pw, x, base);
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) sm[threadIdx.x] = sm[threadIdx.x] + sm[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) block_sums[blockIdx.x] = sm[0];
+}
+// kBatch: blockIdx.y selects the row of n values at v + row * n, whose sum goes to out[row]
+template <class Fr, bool kBatch = false>
+__global__ void __launch_bounds__(256) k_sum_reduce(const Fr* __restrict__ v, size_t n, Fr* __restrict__ out) {
+  __shared__ Fr sm[256];
+  if (kBatch) {
+    v += (size_t)blockIdx.y * n;
+    out += blockIdx.y;
+  }
+  Fr acc = Fr::zero();
+  for (size_t i = threadIdx.x; i < n; i += 256) acc = acc + v[i];
+  sm[threadIdx.x] = acc;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) sm[threadIdx.x] = sm[threadIdx.x] + sm[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = sm[0];
+}
+
+// kBatch (both passes): blockIdx.y selects the polynomial, rows of n at c, t, s and q; its tables start at
+// pw_inv / pw + row * pw_len and its point is their entry 0; the remainder goes to rem[row]
+template <class Fr, bool kBatch = false>
+__global__ void __launch_bounds__(256) k_syndiv_pre(const Fr* __restrict__ c, size_t n, const Fr* __restrict__ pw_inv,
+                                                    Fr zinv, Fr* __restrict__ t, uint32_t pw_len = 0) {
+  if (kBatch) {
+    c += (size_t)blockIdx.y * n;
+    t += (size_t)blockIdx.y * n;
+    pw_inv += (size_t)blockIdx.y * pw_len;
+    zinv = pw_inv[0];
+  }
+  syndiv_pre_chunk<Fr>(c, n, pw_inv, zinv, t, ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E);
+}
+// kBatch: an item whose point is 0 takes its quotient from its coefficients c instead (syndiv_zero_chunk)
+template <class Fr, bool kBatch = false>
+__global__ void __launch_bounds__(256) k_syndiv_post(const Fr* __restrict__ s, size_t n, const Fr* __restrict__ pw, Fr z,
+                                                     Fr* __restrict__ q, Fr* __restrict__ rem, uint32_t pw_len = 0,
+                                                     const Fr* __restrict__ c = nullptr) {
+  const size_t base = ((size_t)blockIdx.x * 256 + threadIdx.x) * EVAL_E;
+  if (kBatch) {
+    const size_t off = (size_t)blockIdx.y * n;
+    s += off;
+    q += off;
+    pw += (size_t)blockIdx.y * pw_len;
+    rem += blockIdx.y;
+    z = pw[0];
+    if (z.is_zero()) {
+      syndiv_zero_chunk<Fr>(c + off, n, q, rem, base);
+      return;
+    }
+  }
+  syndiv_post_chunk<Fr>(s, n, pw, z, q, rem, base);
+}
+
+template <class Fr>
+__global__ void __launch_bounds__(256) k_poly_fold(const Fr* __restrict__ polys, size_t n, size_t batch, Fr gamma,
+                                                   Fr* __restrict__ out) {
+  const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) out[j] = poly_fold_coeff<Fr>(polys, n, batch, gamma, j);
 }
 #endif
 

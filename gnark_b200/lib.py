@@ -40,6 +40,7 @@ EXPORTS = [
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
     "b200_points_ntt", "b200_msm_indexed", "b200_msm_batch", "b200_ntt_batch", "b200_groth16_prove_batch",
+    "b200_poly_eval_batch", "b200_kzg_open_batch", "b200_kzg_fold_open",
 ]
 COMM_ID_BYTES = 128
 
@@ -160,6 +161,10 @@ def load(path: str = None):
         lib.b200_msm_indexed.argtypes = [vp, vp, sz, i32, vp, i32, vp]
     if "b200_msm_batch" not in missing:
         lib.b200_msm_batch.argtypes = [vp, sz, sz, sz, vp, i32, vp]
+    if "b200_kzg_open_batch" not in missing:
+        lib.b200_poly_eval_batch.argtypes = [i32, i32, vp, sz, sz, i32, vp, vp]
+        lib.b200_kzg_open_batch.argtypes = [vp, vp, sz, sz, i32, vp, vp, vp]
+        lib.b200_kzg_fold_open.argtypes = [vp, vp, sz, sz, i32, vp, vp, vp]
     if "b200_table_upload_encoded" not in missing:
         lib.b200_table_upload_encoded.argtypes = [i32, i32, i32, vp, sz, i32, i32, ctypes.POINTER(vp)]
     if "b200_plonk_set_qk" not in missing:
@@ -435,6 +440,29 @@ class Table:
             raise ValueError(f"msm_batch: {total} scalar words for {batch} rows of {n} scalars")
         out = np.zeros((batch, 3 * self.coord_limbs), dtype=np.uint64)
         check(load().b200_msm_batch(self.handle, off, n, batch, ptr(scalars), 1 if sc_dev else 0, ptr(out)))
+        return out
+
+    def kzg_open_batch(self, polys, points, on_device: bool = False):
+        """kzg.Open of every row on this G1 SRS: polys (batch, n, fr_limbs) host array or contiguous device tensor
+        (on_device), points (batch, fr_limbs) Montgomery, one per row.  Returns (values (batch, fr_limbs) = p_b(z_b),
+        proofs (batch, 3 * coord_limbs) Jacobian commitments of (p_b - p_b(z_b)) / (X - z_b) over srs[0, n - 1))."""
+        polys, batch, n = _poly_rows(polys, self.fr_limbs, on_device)
+        points = _fr_rows(points, batch, self.fr_limbs, "kzg_open_batch: points")
+        values = np.zeros((batch, self.fr_limbs), dtype=np.uint64)
+        proofs = np.zeros((batch, 3 * self.coord_limbs), dtype=np.uint64)
+        check(load().b200_kzg_open_batch(self.handle, ptr(polys), n, batch, 1 if on_device else 0, ptr(points),
+                                         ptr(values), ptr(proofs)))
+        return values, proofs
+
+    def kzg_fold_open(self, polys, z, gamma, on_device: bool = False) -> np.ndarray:
+        """kzg.BatchOpenSinglePoint's H: the Jacobian commitment of (f - f(z)) / (X - z), f = sum_b gamma^b polys[b];
+        polys as for kzg_open_batch, z and gamma one fr.Element each (Montgomery)."""
+        polys, batch, n = _poly_rows(polys, self.fr_limbs, on_device)
+        z = _fr_rows(z, 1, self.fr_limbs, "kzg_fold_open: z")
+        gamma = _fr_rows(gamma, 1, self.fr_limbs, "kzg_fold_open: gamma")
+        out = np.zeros(3 * self.coord_limbs, dtype=np.uint64)
+        check(load().b200_kzg_fold_open(self.handle, ptr(polys), n, batch, 1 if on_device else 0, ptr(z), ptr(gamma),
+                                        ptr(out)))
         return out
 
     def msm_async(self, d_scalars, d_out, off: int = 0, n: int = None):
@@ -755,6 +783,36 @@ def plonk_build_z(domain0: "Domain", d_l, d_r, d_o, d_perm, beta, gamma, d_z):
 def poly_eval(dev, curve, d_coeffs, n, x) -> np.ndarray:
     out = np.zeros(CURVE_SHAPES[curve][0], dtype=np.uint64)
     check(load().b200_poly_eval(dev, curve, ptr(d_coeffs), n, ptr(x), ptr(out)))
+    return out
+
+
+def _poly_rows(polys, fr_limbs, on_device):
+    """(polys, batch, n) of a (batch, n, fr_limbs) host array or contiguous device tensor"""
+    if on_device:
+        if not polys.is_contiguous():
+            raise ValueError("the device polynomials must be contiguous")
+    else:
+        polys = np.ascontiguousarray(polys, dtype=np.uint64)
+    if len(polys.shape) != 3 or int(polys.shape[2]) != fr_limbs:
+        raise ValueError(f"polynomials must be shaped (batch, n, {fr_limbs}), not {tuple(polys.shape)}")
+    return polys, int(polys.shape[0]), int(polys.shape[1])
+
+
+def _fr_rows(a, rows, fr_limbs, what):
+    a = np.ascontiguousarray(a, dtype=np.uint64)
+    if a.size != rows * fr_limbs:
+        raise ValueError(f"{what}: {a.size} words for {rows} fr.Elements")
+    return a
+
+
+def poly_eval_batch(dev, curve, polys, points, on_device: bool = False) -> np.ndarray:
+    """values[b] = polys[b](points[b]) for every row: polys (batch, n, fr_limbs) host array or contiguous device tensor
+    (on_device), points (batch, fr_limbs) Montgomery on the host.  Returns (batch, fr_limbs)."""
+    frl = CURVE_SHAPES[curve][0]
+    polys, batch, n = _poly_rows(polys, frl, on_device)
+    points = _fr_rows(points, batch, frl, "poly_eval_batch: points")
+    out = np.zeros((batch, frl), dtype=np.uint64)
+    check(load().b200_poly_eval_batch(dev, curve, ptr(polys), n, batch, 1 if on_device else 0, ptr(points), ptr(out)))
     return out
 
 

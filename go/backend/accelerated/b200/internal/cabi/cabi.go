@@ -379,6 +379,67 @@ func (t *Table) MSMBatch(off, n, batch int, scalars, out unsafe.Pointer) error {
 	})
 }
 
+// KZGOpenBatch is b200_kzg_open_batch on a G1 SRS table: kzg.Open of `batch` polynomials of n coefficients (polys,
+// item-major, on the device when onDev, else host memory borrowed for the call) at points (batch fr.Elements); values
+// (batch fr.Elements) and proofs (batch G1Jac) are host memory.
+func (t *Table) KZGOpenBatch(polys unsafe.Pointer, n, batch int, onDev bool, points, values, proofs unsafe.Pointer) error {
+	return Call(func() int32 {
+		return int32(C.b200_kzg_open_batch(t.h, polys, C.size_t(n), C.size_t(batch), boolInt(onDev), points, values, proofs))
+	})
+}
+
+// KZGFoldOpen is b200_kzg_fold_open: the H of kzg.BatchOpenSinglePoint (one G1Jac to proof) of `batch` polynomials of
+// n coefficients folded with powers of gamma, opened at z.
+func (t *Table) KZGFoldOpen(polys unsafe.Pointer, n, batch int, onDev bool, z, gamma, proof unsafe.Pointer) error {
+	return Call(func() int32 {
+		return int32(C.b200_kzg_fold_open(t.h, polys, C.size_t(n), C.size_t(batch), boolInt(onDev), z, gamma, proof))
+	})
+}
+
+// PolyEvalBatch is b200_poly_eval_batch: values[b] = p_b(points[b]) for `batch` polynomials of n coefficients.
+func PolyEvalBatch(dev int, curve int32, polys unsafe.Pointer, n, batch int, onDev bool, points, values unsafe.Pointer) error {
+	return Call(func() int32 {
+		return int32(C.b200_poly_eval_batch(C.int32_t(dev), C.int32_t(curve), polys, C.size_t(n), C.size_t(batch),
+			boolInt(onDev), points, values))
+	})
+}
+
+// DeviceBuffer is device memory from b200_alloc, filled from host memory with b200_h2d.
+type DeviceBuffer struct {
+	dev int
+	P   unsafe.Pointer
+}
+
+// Upload copies `bytes` bytes of host memory (borrowed for the call) into a new device buffer on dev.
+func Upload(dev int, src unsafe.Pointer, bytes int) (*DeviceBuffer, error) {
+	b := &DeviceBuffer{dev: dev}
+	if err := Call(func() int32 { return int32(C.b200_alloc(C.int32_t(dev), C.size_t(bytes), &b.P)) }); err != nil {
+		return nil, err
+	}
+	if bytes > 0 {
+		if err := Call(func() int32 { return int32(C.b200_h2d(C.int32_t(dev), b.P, src, C.size_t(bytes))) }); err != nil {
+			b.Free()
+			return nil, err
+		}
+	}
+	return b, nil
+}
+
+// Free is b200_free; safe on a nil buffer and more than once.
+func (b *DeviceBuffer) Free() {
+	if b != nil && b.P != nil {
+		C.b200_free(C.int32_t(b.dev), b.P)
+		b.P = nil
+	}
+}
+
+func boolInt(v bool) C.int32_t {
+	if v {
+		return 1
+	}
+	return 0
+}
+
 // Free is b200_table_free; safe on a nil table and more than once.
 func (t *Table) Free() {
 	if t != nil && t.h != nil {

@@ -319,6 +319,30 @@ int32_t b200_poly_eval(int32_t dev, int32_t curve, const void* d_coeffs, size_t 
 int32_t b200_poly_div_by_linear(int32_t dev, int32_t curve, void* d_coeffs, size_t n, const void* z_mont,
                                 void* claimed_value_host);
 
+/* ---- KZG over a G1 SRS table (kzg_host.cu; gnark-crypto's kzg.Commit / Open / BatchOpenSinglePoint) ----
+ * A commitment needs no entry point of its own: kzg.Commit(p) is b200_msm on the SRS table, and a batch of commitments
+ * is ONE b200_msm_batch on it (off = 0, n = the longest polynomial, the shorter ones zero-padded).
+ * The three calls below are synchronous, synchronise once at the end and join pending pipelined MSMs first.  polys:
+ * batch * n fr.Elements (Montgomery), item-major, on the host or the device (polys_on_dev); they are only read.  The
+ * caller zero-pads shorter polynomials to n, which changes no commitment, value or quotient.  points / z / gamma: on the
+ * host; a point may be 0.  Refusals, each checked before anything is allocated, naming the argument or the limit, with
+ * every output untouched: a null pointer, a G2 table, n - 1 above the table's point count, batch * n overflowing, and the
+ * quotient MSM's limits (batch * (n - 1) * windows < 2^31, batch * bucket sets * 2^(c-1) < 2^31 - 1; the message names the
+ * largest batch that fits).  batch = 0 writes nothing; n = 0 gives value 0 and the point at infinity, n = 1 value c_0 and
+ * the point at infinity. */
+/* values[b] = p_b(points[b]), b < batch: batch fr.Elements to values_host */
+int32_t b200_poly_eval_batch(int32_t dev, int32_t curve, const void* polys, size_t n, size_t batch, int32_t polys_on_dev,
+                             const void* points_mont, void* values_host);
+/* kzg.Open of every item: values[b] = p_b(z_b), proofs[b] = sum_{i<n-1} q_b[i] * srs[i] (G1Jac, gnark layout) with
+ * q_b = (p_b - p_b(z_b)) / (X - z_b).  One batched division and one batched MSM over srs[0, n - 1): an SRS of exactly
+ * n - 1 points is enough, as for kzg.Open.  The MSM window is a precomputed table's own, else that of an n-point MSM. */
+int32_t b200_kzg_open_batch(b200_table_t srs, const void* polys, size_t n, size_t batch, int32_t polys_on_dev,
+                            const void* points_mont, void* values_host, void* proofs_jac_host);
+/* kzg.BatchOpenSinglePoint's H: f = sum_b gamma^b p_b (gamma^0 = 1), proof = Commit((f - f(z)) / (X - z)) over
+ * srs[0, n - 1), one G1Jac.  The claimed values come from b200_poly_eval_batch on the same polynomials. */
+int32_t b200_kzg_fold_open(b200_table_t srs, const void* polys, size_t n, size_t batch, int32_t polys_on_dev,
+                           const void* z_mont, const void* gamma_mont, void* proof_jac_host);
+
 /* ---- PLONK prover (host orchestration in C++, plonk_host.cu; the reference has no accelerated PLONK - this is
  *      the device-resident twin of backend/plonk/bn254/prove.go:98-837 behind one call, for a Go package
  *      backend/accelerated/b200/plonk mirroring backend/plonk/plonk.go:94-135).
