@@ -8,6 +8,7 @@
 #include "capi_common.h"
 #include "file_stage.h"
 #include "fixed_base.cuh"
+#include "points_scale.cuh"
 
 namespace gb200 {
 
@@ -433,6 +434,11 @@ static int32_t table_finish(DeviceCtx* ctx, b200_table_s* t) {
   CK(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
+// the error of a failed point decode: status = {DECODE_* code, index of the point}
+static int32_t decode_failure(const char* what, const uint32_t status[2]) {
+  static const char* why[] = {"", "invalid metadata bits", "coordinate not reduced modulo p", "point not on the curve"};
+  return set_error(std::string(what) + ": point " + std::to_string(status[1]) + ": " + why[status[0] < 4 ? status[0] : 0]);
+}
 }  // namespace gb200
 
 extern "C" {
@@ -482,10 +488,7 @@ int32_t b200_table_upload_encoded(int32_t dev, int32_t curve, int32_t group, con
     if (e != cudaSuccess) return cuda_fail("points decode", e);
     rc = st.finish("table_upload_encoded", 0);
     if (rc) return rc;
-    if (status[0]) {
-      static const char* why[] = {"", "invalid metadata bits", "coordinate not reduced modulo p", "point not on the curve"};
-      return set_error(std::string("table_upload_encoded: point ") + std::to_string(status[1]) + ": " + why[status[0] < 4 ? status[0] : 0]);
-    }
+    if (status[0]) return decode_failure("table_upload_encoded", status);
   }
   rc = table_finish(ctx, t.get()); if (rc) return rc;
   *out = t.release();
@@ -810,6 +813,63 @@ int32_t b200_points_ntt(b200_domain_t d, int32_t group, void* points_affine, int
   void* buf;
   CK(st.inout(points_affine, ((size_t)1 << d->logn) * ops->affine_bytes, points_on_dev, &buf));
   return st.finish("points_ntt", ops->points_ntt(ctx->stream, d->impl, buf, inverse));
+  GUARD_END
+}
+
+// points[i] <- (c * t^i) * points[i] (points_scale.cuh): the point vectors of a Groth16 MPC contribution
+int32_t b200_points_scale(int32_t dev, int32_t curve, int32_t group, void* points_affine, size_t n, int32_t points_on_dev,
+                          const void* c_mont, const void* t_mont) {
+  GUARD_BEGIN
+  if (curve < 0 || curve > 3) return set_error("points_scale: unknown curve " + std::to_string(curve));
+  if (group != 1 && group != 2) return set_error("points_scale: unknown group " + std::to_string(group) + " (1 = G1, 2 = G2)");
+  if (!c_mont) return set_error("points_scale: null c");
+  if (n && !points_affine) return set_error("points_scale: null points");
+  if (n > PS_MAX_POINTS) return set_error("points_scale: n = " + std::to_string(n) + " exceeds the kernel's 32-bit point indices");
+  GB_DEVICE(ctx, dev);
+  const MsmOps* ops = get_msm_ops(curve, group);
+  if (!ops || !ops->points_scale) return set_error("points_scale: unsupported curve/group");
+  if (n == 0) return 0;
+  int32_t rc = msm_join(ctx); if (rc) return rc;
+  Staging st(ctx);
+  void* buf;
+  CK(st.inout(points_affine, n * ops->affine_bytes, points_on_dev, &buf));
+  return st.finish("points_scale", ops->points_scale(ctx->stream, buf, n, c_mont, t_mont));
+  GUARD_END
+}
+
+// n encoded points -> n affine points (the decoder of b200_table_upload_encoded).  The points are decoded into a scratch
+// buffer and copied out only when every one of them is valid, so a failure leaves out_affine untouched.
+int32_t b200_points_decode(int32_t dev, int32_t curve, int32_t group, const void* bytes, size_t n, int32_t encoding,
+                           void* out_affine, int32_t out_on_dev) {
+  GUARD_BEGIN
+  if (curve < 0 || curve > 3) return set_error("points_decode: unknown curve " + std::to_string(curve));
+  if (group != 1 && group != 2) return set_error("points_decode: unknown group " + std::to_string(group) + " (1 = G1, 2 = G2)");
+  if (encoding != B200_POINTS_RAW && encoding != B200_POINTS_COMPRESSED)
+    return set_error("points_decode: unknown encoding " + std::to_string(encoding) + " (1 = raw, 2 = compressed)");
+  if (n && !bytes) return set_error("points_decode: null bytes");
+  if (n && !out_affine) return set_error("points_decode: null out");
+  if (n > 0xffffffffull) return set_error("points_decode: n = " + std::to_string(n) + " exceeds the decoder's 32-bit point indices");
+  GB_DEVICE(ctx, dev);
+  const MsmOps* ops = get_msm_ops(curve, group);
+  if (!ops) return set_error("points_decode: unsupported curve/group");
+  const size_t per = ops->encoded_bytes(encoding);
+  if (per == 0) return set_error("points_decode: encoding not supported for this group");
+  if (n == 0) return 0;
+  Staging st(ctx);
+  uint32_t status[2] = {0, 0};
+  const void* d_bytes;
+  void *d_pts, *d_status;
+  CK(st.in(bytes, n * per, false, &d_bytes));
+  CK(st.scratch(n * ops->affine_bytes, &d_pts));
+  CK(st.scratch(sizeof(status), &d_status));
+  CK(cudaMemsetAsync(d_status, 0, sizeof(status), ctx->stream));
+  cudaError_t e = ops->decode(ctx->stream, d_bytes, n, encoding, curve, group, d_pts, (uint32_t*)d_status);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(status, d_status, sizeof(status), cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) return st.finish("points_decode", e);
+  if (status[0]) return st.finish("points_decode", decode_failure("points_decode", status));
+  st.download(out_affine, d_pts, n * ops->affine_bytes, out_on_dev);
+  return st.finish("points_decode", 0);
   GUARD_END
 }
 

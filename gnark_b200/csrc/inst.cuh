@@ -10,9 +10,13 @@
 #include "ntt_impl.cuh"
 #include "plonk.cuh"
 #include "points_ntt.cuh"
+#include "points_scale.cuh"
 #include "../../include/gnark_b200.h"
 
 namespace gb200 {
+
+template <class Fr>
+struct NttInst;   // below: MsmInst::points_scale builds its scalars with NttInst<Fr>::scale_powers
 
 // ---------------------------------------------------------------------------
 // MSM
@@ -89,9 +93,25 @@ struct MsmInst {
                                                                        reinterpret_cast<Affine<F>*>(d_out_affine), d_status);
     return cudaGetLastError();
   }
+  // points_scale.cuh: d_points[i] <- (c * t^i) * d_points[i], i < n <= PS_MAX_POINTS; t null means t = 1
+  static cudaError_t points_scale(cudaStream_t st, void* d_points, size_t n, const void* c_mont, const void* t_mont) {
+    if (n == 0) return cudaSuccess;
+    AsyncBuf kb;
+    GB_CUDA_TRY(kb.alloc(n * sizeof(Fr), st));
+    Fr* k = reinterpret_cast<Fr*>(kb.p);
+    k_points_scale_ones<Fr><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(k, n);
+    GB_CUDA_TRY(cudaGetLastError());
+    const Fr one = Fr::one();
+    GB_CUDA_TRY(NttInst<Fr>::scale_powers(st, k, n, c_mont, t_mont ? t_mont : &one));
+    k_points_scale<Fr, F><<<(unsigned)((n + PS_THREADS - 1) / PS_THREADS), PS_THREADS, 0, st>>>(
+        reinterpret_cast<Affine<F>*>(d_points), k, (uint32_t)n);
+    GB_CUDA_TRY(cudaGetLastError());
+    return kb.release_on(st);
+  }
   static const MsmOps* ops() {
     static const MsmOps o = {Fr::Params::BITS, sizeof(Fr), sizeof(Affine<F>), sizeof(Jacobian<F>), &ws_bytes, &run,
-                             &precompute, &acc_blocks_per_sm, &fixed_base, &fold, &encoded_bytes, &decode, nullptr};
+                             &precompute, &acc_blocks_per_sm, &fixed_base, &fold, &encoded_bytes, &decode, nullptr,
+                             &points_scale};
     return &o;
   }
   // G1 only: the group NTT is instantiated through ops_g1(), so G2 compiles none of its kernels

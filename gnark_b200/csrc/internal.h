@@ -71,6 +71,9 @@ struct MsmOps {
   // group-element NTT (points_ntt.cuh) in place on the 2^logn device points of d_points, on the NttDomainDev of the same
   // curve's Fr behind `dom`; G1 only (null for G2)
   cudaError_t (*points_ntt)(cudaStream_t st, void* dom, void* d_points, int inverse);
+  // variable-base scaling (points_scale.cuh) in place on n <= PS_MAX_POINTS device points: d_points[i] <- (c * t^i) *
+  // d_points[i]; c, t: one Fr element each on the host (Montgomery), t null means t = 1
+  cudaError_t (*points_scale)(cudaStream_t st, void* d_points, size_t n, const void* c_mont, const void* t_mont);
 };
 
 struct NttOps {

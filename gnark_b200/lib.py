@@ -40,7 +40,7 @@ EXPORTS = [
     "b200_points_allreduce", "b200_msm_allreduce", "b200_msm_submit_dev", "b200_plonk_last_stage_ms", "b200_points_fold",
     "b200_plonk_set_qk", "b200_plonk_set_quotient_randomizers", "b200_table_upload_encoded", "b200_msm_gather", "b200_pedersen_key_load", "b200_pedersen_key_free", "b200_pedersen_commit", "b200_pedersen_fold",
     "b200_points_ntt", "b200_msm_indexed", "b200_msm_batch", "b200_ntt_batch", "b200_groth16_prove_batch",
-    "b200_poly_eval_batch", "b200_kzg_open_batch", "b200_kzg_fold_open",
+    "b200_poly_eval_batch", "b200_kzg_open_batch", "b200_kzg_fold_open", "b200_points_scale", "b200_points_decode",
 ]
 COMM_ID_BYTES = 128
 
@@ -195,6 +195,9 @@ def load(path: str = None):
         lib.b200_ntt_batch.argtypes = [vp, vp, sz, i32, i32, i32, i32]
     if "b200_points_ntt" not in missing:
         lib.b200_points_ntt.argtypes = [vp, i32, vp, i32, i32]
+    if "b200_points_scale" not in missing:
+        lib.b200_points_scale.argtypes = [i32, i32, i32, vp, sz, i32, vp, vp]
+        lib.b200_points_decode.argtypes = [i32, i32, i32, vp, sz, i32, vp, i32]
     lib.b200_groth16_compute_h.argtypes = [vp, vp, vp, vp, sz, i32, vp, i32]
     lib.b200_vec_op.argtypes = [i32, i32, i32, vp, vp, vp, sz]
     lib.b200_vec_bit_reverse.argtypes = [i32, i32, vp, u32]
@@ -581,6 +584,33 @@ def fixed_base_batch(curve: int, group: int, base_affine: np.ndarray, scalars, n
         out = np.zeros((n, 2 * cl), dtype=np.uint64)
     check(load().b200_fixed_base_batch(dev, curve, group, ptr(base_affine), ptr(scalars), 1 if on_dev else 0, n,
                                        ptr(out), 1 if hasattr(out, "data_ptr") else 0))
+    return out
+
+
+def points_scale(curve: int, group: int, points, c, t=None, n: int = None, dev: int = 0):
+    """points[i] <- (c * t^i) * points[i] in place (t None: t = 1), the point vectors of a Groth16 MPC contribution
+    (mpcsetup phase1.go SrsCommons.update, phase2.go Phase2.update).  points: affine points in gnark layout, a host numpy
+    array or a device tensor (anything with data_ptr()); c, t: one fr.Element each (Montgomery limbs).  Returns points."""
+    frl, fpl, deg = CURVE_SHAPES[curve]
+    cl = fpl * (deg if group == 2 else 1)
+    on_dev = hasattr(points, "data_ptr")
+    if n is None:
+        n = (points.numel() if on_dev else points.size) // (2 * cl)
+    c = np.ascontiguousarray(c, dtype=np.uint64)
+    t = None if t is None else np.ascontiguousarray(t, dtype=np.uint64)
+    check(load().b200_points_scale(dev, curve, group, ptr(points), n, 1 if on_dev else 0, ptr(c), ptr(t)))
+    return points
+
+
+def points_decode(curve: int, group: int, data, n: int, encoding: int, dev: int = 0, out=None):
+    """n points in gnark-crypto's serialised encoding (POINTS_RAW / POINTS_COMPRESSED, fixed size per point) -> affine
+    points in gnark layout, decoded on the device.  out: a host numpy array (default) or a device tensor; returns out."""
+    frl, fpl, deg = CURVE_SHAPES[curve]
+    cl = fpl * (deg if group == 2 else 1)
+    if out is None:
+        out = np.zeros((n, 2 * cl), dtype=np.uint64)
+    buf = np.frombuffer(bytes(data), dtype=np.uint8).copy() if n else np.zeros(1, dtype=np.uint8)
+    check(load().b200_points_decode(dev, curve, group, ptr(buf), n, encoding, ptr(out), 1 if hasattr(out, "data_ptr") else 0))
     return out
 
 

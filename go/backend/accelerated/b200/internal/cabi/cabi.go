@@ -339,6 +339,32 @@ func PointsNTT(dev int, curve int32, log2n uint32, points unsafe.Pointer, invers
 	return Call(func() int32 { return int32(C.b200_points_ntt(d, 1, points, 0, inv)) })
 }
 
+// PointsScale is b200_points_scale: points[i] <- (c * t^i) * points[i], i < n, in place on n affine points of G1
+// (group 1) or G2 (group 2) of `curve` in host memory; c and t point to one fr.Element each, t nil means t = 1.
+func PointsScale(dev int, curve, group int32, points unsafe.Pointer, n int, c, t unsafe.Pointer) error {
+	return Call(func() int32 {
+		return int32(C.b200_points_scale(C.int32_t(dev), C.int32_t(curve), C.int32_t(group), points, C.size_t(n), 0, c, t))
+	})
+}
+
+// Encodings of b200_points_decode.
+const (
+	PointsRaw        = int32(C.B200_POINTS_RAW)
+	PointsCompressed = int32(C.B200_POINTS_COMPRESSED)
+)
+
+// PointsDecode is b200_points_decode: n points in gnark-crypto's fixed-size encoding (PointsRaw / PointsCompressed) to n
+// affine points of G1 or G2 in host memory at out.
+func PointsDecode(dev int, curve, group int32, data []byte, n int, encoding int32, out unsafe.Pointer) error {
+	if n == 0 {
+		return nil
+	}
+	return Call(func() int32 {
+		return int32(C.b200_points_decode(C.int32_t(dev), C.int32_t(curve), C.int32_t(group), unsafe.Pointer(&data[0]),
+			C.size_t(n), C.int32_t(encoding), out, 0))
+	})
+}
+
 // Table is a device-resident MSM base table (b200_table_t).
 type Table struct {
 	h C.b200_table_t

@@ -254,6 +254,35 @@ int32_t b200_ntt_batch(b200_domain_t d, void* data, size_t batch, int32_t data_o
  * Synchronous.  group must be 1: G2 is not supported. */
 int32_t b200_points_ntt(b200_domain_t d, int32_t group, void* points_affine, int32_t points_on_dev, int32_t inverse);
 
+/* ---- Groth16 MPC contributions (SURVEY.md §8(f)-3) ----------------------------------------------------------------
+ * Every step of a contribution to gnark's ceremony (backend/groth16/<curve>/mpcsetup) is out[i] = (c * t^i) * P[i]:
+ *   phase 1, SrsCommons.update (phase1.go:104-147), domain size N:
+ *     G1.Tau[1 .. 2N-2] and G2.Tau[1 .. N-1]   (c, t) = (tau', tau')
+ *     G1.AlphaTau[0 .. N-1]                     (c, t) = (alpha', tau')
+ *     G1.BetaTau[0 .. N-1]                      (c, t) = (beta', tau')     (and the single point G2.Beta *= beta')
+ *   phase 2, Phase2.update (phase2.go:110-135):
+ *     G1.Z, G1.PKK                              c = 1/delta', t = 1
+ *     G1.SigmaCKK[j]                            c = sigma_j, t = 1         (and G1.Delta, G2.Delta, G2.Sigma[j])
+ * b200_points_scale: points[i] <- (c * t^i) * points[i], i < n (t^0 = 1; t = NULL means t = 1), in place on n affine
+ * points of G1 or G2 of `curve` (group 1 or 2; BW6-761's G2 is over Fp), host or device buffer.  c, t: one fr.Element
+ * each (Montgomery) on the host.  The scalars are built on the device (b200_vec_scale_powers' kernel on a vector of
+ * ones); one thread per point runs a double-and-add with mixed additions over the canonical scalar, and the
+ * results are canonical affine points ((0,0) = infinity).  Points are not checked to be on the curve, as with gnark's
+ * ScalarMultiplication.  n = 0 does nothing; c = 0 gives n points at infinity.  Synchronous; joins pending pipelined
+ * MSMs first.  Refused before anything is launched, with the argument named and the buffer untouched: an unknown curve or
+ * group, a null c, null points with n > 0, n >= 2^32. */
+int32_t b200_points_scale(int32_t dev, int32_t curve, int32_t group, void* points_affine, size_t n, int32_t points_on_dev,
+                          const void* c_mont, const void* t_mont);
+/* n points in gnark-crypto's serialised encoding (B200_POINTS_RAW / B200_POINTS_COMPRESSED, as for
+ * b200_table_upload_encoded: what the Encoder writes for each point of SrsCommons and Phase2, marshal.go:19-57,157-179)
+ * -> n affine points in gnark layout, out_affine on the host or the device.  bytes: n * (point size) bytes on the host.
+ * The decoder of b200_table_upload_encoded, with its checks: canonical coordinates and, except for raw G2, on the curve;
+ * subgroup membership is not checked, as with UnsafeReadFrom.  An invalid point fails the call, names its index and
+ * leaves out_affine untouched.  Refused before anything is launched: an unknown curve, group or encoding, null
+ * bytes or out with n > 0, n >= 2^32.  n = 0 does nothing.  Synchronous. */
+int32_t b200_points_decode(int32_t dev, int32_t curve, int32_t group, const void* bytes, size_t n, int32_t encoding,
+                           void* out_affine, int32_t out_on_dev);
+
 /* ---- Groth16 quotient (replaces computeH icicle.go:1391-1488; CPU twin
  *      prove.go:346-389).  a,b,c: `len` fr.Elements each (len <= n, zero padded
  *      internally); h_out: n elements, BIT-REVERSED order, Montgomery - directly
